@@ -200,6 +200,17 @@ int promp_process_samples_ragged(int M, int max_paths, int max_samples, int obs_
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * Launch geometry of the processing kernel for one shape, computed on the host (no CUDA call).  It replaces no reference
+ * function: it exists so that tests can name the code path a shape exercises.  Fixed horizon (ragged = 0): max_paths = E,
+ * NS = E*H, as in promp_process_samples.  Variable-length paths (ragged = 1): max_paths and NS = max_samples as in
+ * promp_process_samples_ragged (promp_baseline_fit: M = 1, max_paths = n_paths, NS = n_samples); H is ignored.
+ *   out [8] host int32: C (trajectory chunks per task), EPC (trajectories per chunk), chunk_cap, finish_cap (samples the
+ *   front / finish stage stages in shared memory; 0 = float64 workspace), tt_cap (steps covered by the t/100 table),
+ *   pred_tile, stage_f, stage_l (1 = that stage keeps its sample arrays in shared memory).
+ */
+int promp_process_launch_info(int M, int max_paths, int H, int obs_dim, int NS, int ragged, int32_t* out);
+
+/*
  * Standalone LinearFeatureBaseline (baselines/linear_baseline.py): fit(paths, target_key) (:55-77) and predict(path)
  * (:17-33) for a flat list of n_paths paths stored back to back (path e = samples [path_off[e], path_off[e+1]), path_off
  * [n_paths+1] int32 device memory; the time feature restarts at 0 in every path, :101-106).

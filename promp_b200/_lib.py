@@ -51,6 +51,7 @@ _SIGNATURES = {
     'promp_process_workspace_bytes_ragged': (c_int64, [c_int, c_int, c_int, c_int]),
     'promp_process_samples_ragged': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_double, c_double, c_double, c_int,
                                              c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P]),
+    'promp_process_launch_info': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'promp_adj_avg_rewards': (c_int, [c_int64, _P, c_double, c_double, _P, _P]),
     'promp_baseline_fit_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'promp_baseline_fit': (c_int, [c_int, c_int, c_int, _P, _P, _P, c_double, _P, _P, _P, c_int64, _P]),

@@ -683,6 +683,10 @@ struct ProcGeom {
 };
 // Shared memory of one CTA when a chunk holds `EPC` paths (front stage: the chunk's rewards + returns; finish stage: the
 // task's rewards + baseline; whichever is larger, because any CTA may turn out to be the finisher).
+// Invariant: !stage_f implies !stage_l.  front - fin = round16(chunk_samples*12) + ring - proc_smem_finish_fixed(Do) - NS*12
+// with chunk_samples <= NS, and the Gram loop's TMA ring (PS_RING*PS_TS*Do*4 B) plus the 12 B of rounding is smaller than
+// the finish stage's fixed arrays for every obs_dim 1..19, so front < fin: when the front stage does not fit, neither does
+// the finish stage.  launch_process therefore has no <false, true> kernel.
 static ProcGeom proc_geom_for(int EPC, int E, int H, int Do, int NS, bool ragged) {
     ProcGeom g;
     g.EPC = EPC;
@@ -743,16 +747,29 @@ static ProcLayout proc_layout(int M, int E, int H, int Do, int NS, bool ragged) 
 static int launch_process(ProcArgs& A, const ProcGeom& g, cudaStream_t stream) {
     A.C = g.C; A.EPC = g.EPC; A.chunk_cap = g.chunk_cap; A.finish_cap = g.finish_cap; A.tt_cap = g.tt_cap;
     A.pred_tile = g.pred_tile;
+    PROMP_REQUIRE(g.stage_f || !g.stage_l, "process_fused_kernel: finish stage staged without a staged front stage "
+                  "(M=%d E=%d Do=%d NS=%d); proc_geom_for's invariant is broken", A.M, A.E, A.Do, A.NS);
     auto kern = g.stage_f ? (g.stage_l ? process_fused_kernel<true, true> : process_fused_kernel<true, false>)
-                          : (g.stage_l ? process_fused_kernel<false, true> : process_fused_kernel<false, false>);
-    static size_t configured[4] = {0, 0, 0, 0};
-    const int which = (g.stage_f ? 2 : 0) + (g.stage_l ? 1 : 0);
+                          : process_fused_kernel<false, false>;
+    static size_t configured[3] = {0, 0, 0};
+    const int which = g.stage_f ? (g.stage_l ? 2 : 1) : 0;
     if (g.smem > configured[which]) {
         PROMP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
         configured[which] = g.smem;
     }
     kern<<<dim3(A.C, A.M), PS_THREADS, g.smem, stream>>>(A);
     PROMP_LAUNCH_CHECK("process_fused_kernel");
+    return PROMP_OK;
+}
+
+extern "C" int promp_process_launch_info(int M, int max_paths, int H, int obs_dim, int NS, int ragged, int32_t* out) {
+    PROMP_REQUIRE(M > 0 && max_paths > 0 && obs_dim > 0 && NS > 0 && out, "promp_process_launch_info: bad arguments");
+    PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "promp_process_launch_info: obs_dim %d too large (max %d)", obs_dim,
+                  (PS_MAXCOL - 5) / 2);
+    PROMP_REQUIRE(ragged || (H > 0 && NS == max_paths * H), "promp_process_launch_info: fixed horizon needs NS = E*H");
+    const ProcGeom g = proc_geom(M, max_paths, ragged ? 0 : H, obs_dim, NS, ragged != 0);
+    const int32_t v[8] = {g.C, g.EPC, g.chunk_cap, g.finish_cap, g.tt_cap, g.pred_tile, g.stage_f ? 1 : 0, g.stage_l ? 1 : 0};
+    for (int i = 0; i < 8; ++i) out[i] = v[i];
     return PROMP_OK;
 }
 
