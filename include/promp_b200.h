@@ -483,6 +483,52 @@ int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N,
                          const float* params, int64_t param_stride, const float* obs, float* mean,
                          void* stream);
 
+/*
+ * Padded policy kernels: any obs_dim in [1, 19], act_dim in [1, 8], hidden 32 or 64 (the policy of
+ * policies/meta_gaussian_mlp_policy.py:9-157 / gaussian_mlp_policy.py:31-184 for any Box observation / action space of those
+ * sizes).  The entry points above are built for the exact (obs_dim, act_dim) = (2,2), (4,2), (17,6) only and reject every
+ * other shape; the *_padded siblings below run kernels instantiated at caps and take the logical sizes at run time.
+ *
+ * Layout.  promp_policy_layout gives out = (obs_cap, act_cap, hidden, P) with P = promp_num_params(obs_cap, act_cap, hidden)
+ * (obs_cap = 8 for obs_dim <= 8, else 20; act_cap = 2 for act_dim <= 2, else 8; P % 4 == 0).  Every parameter-shaped vector
+ * of the padded entries (params, grad, out_params, vec, out, skip_theta, theta_copy_out: [.., P]) is the flat layout of
+ * promp_num_params at the caps, in the same order W0[obs_cap,H] b0[H] W1[H,H] b1[H] W2[H,act_cap] b2[act_cap]
+ * log_std[act_cap], with the logical parameters in W0[:obs_dim, :], W2[:, :act_dim], b2[:act_dim], log_std[:act_dim].
+ * Zero-pad invariant: every other entry (pad rows of W0, pad columns of W2, pad entries of b2 / log_std) must be 0 on input;
+ * the kernels then return exactly 0 for them in every gradient and in the Hessian-vector product (out = vec there), so SGD,
+ * Adam, CG / TRPO and the meta-update keep them at 0.
+ * Data.  obs [M,N,obs_dim], act / old_mean / old_log_std / mean with act_dim columns: the logical sizes, as for the exact
+ * entries.  promp_policy_layout is host-only; it returns PROMP_ERR_INVALID_ARG (and sets promp_last_error) out of range.
+ * The *_padded siblings take the arguments of the entry named without the suffix and replace the same reference functions.
+ * They always run the padded instantiations, also for shapes the exact table covers.
+ */
+int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]);
+int64_t promp_policy_workspace_bytes_padded(int M, int N, int obs_dim, int act_dim, int hidden);
+int promp_policy_forward_padded(int obs_dim, int act_dim, int hidden, int M, int N,
+                                const float* params, int64_t param_stride, const float* obs, float* mean,
+                                void* stream);
+int promp_policy_grad_ex_padded(int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid, const float* params,
+                                int64_t param_stride, const float* obs, const float* act, const float* adv, const float* old_mean,
+                                const float* old_log_std, int ls_per_sample, int obj_kind, float obj_scale, float clip_eps,
+                                float kl_coeff, int clip_log_std, float min_log_std, float* grad, float* out_params, float sgd_lr,
+                                float* stats, const int32_t* skip_flag, const float* skip_theta, int32_t* unclipped_out,
+                                float* theta_copy_out, void* workspace, int64_t workspace_bytes, void* stream);
+int promp_policy_hvp_ragged_padded(int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
+                                   const float* params, int64_t param_stride,
+                                   const float* obs, const float* act, const float* adv,
+                                   const float* old_mean, const float* old_log_std, int ls_per_sample,
+                                   int obj_kind, float inner_lr, float kl_coeff,
+                                   int clip_log_std, float min_log_std,
+                                   const float* vec, float* out, float* stats,
+                                   void* workspace, int64_t workspace_bytes, void* stream);
+int64_t promp_policy_chain_workspace_bytes_padded(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                                  const promp_policy_stage* stages);
+int promp_policy_chain_num_launches_padded(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                           const promp_policy_stage* stages);
+int promp_policy_chain_padded(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
+                              const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
+                              void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

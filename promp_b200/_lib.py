@@ -82,6 +82,17 @@ _SIGNATURES = {
     'promp_trpo_step': (c_int, [c_int, _P, _P, c_float, c_float, _P, c_float, _P, _P, _P]),
     'promp_trpo_select': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P, _P, _P]),
     'promp_policy_forward': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P]),
+    'promp_policy_layout': (c_int, [c_int, c_int, c_int, _P]),
+    'promp_policy_workspace_bytes_padded': (c_int64, [c_int, c_int, c_int, c_int, c_int]),
+    'promp_policy_forward_padded': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P]),
+    'promp_policy_grad_ex_padded': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P, _P, c_int, c_int,
+                                            c_float, c_float, c_float, c_int, c_float, _P, _P, c_float, _P, _P, _P, _P, _P, _P,
+                                            c_int64, _P]),
+    'promp_policy_hvp_ragged_padded': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, c_int64, _P, _P, _P, _P, _P, c_int,
+                                               c_int, c_float, c_float, c_int, c_float, _P, _P, _P, _P, c_int64, _P]),
+    'promp_policy_chain_workspace_bytes_padded': (c_int64, [c_int, c_int, c_int, c_int, c_int, _P]),
+    'promp_policy_chain_num_launches_padded': (c_int, [c_int, c_int, c_int, c_int, c_int, _P]),
+    'promp_policy_chain_padded': (c_int, [c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int64, _P]),
     'promp_set_option': (c_int, [c_char_p, c_int]),
     'promp_comm_buffer_bytes': (c_int64, [c_int, c_int]),
     'promp_comm_alloc': (c_int, [c_int64, _P]),
@@ -164,3 +175,11 @@ def set_option(name, value):
 
 def call(name, *args):
     check(getattr(load(), name)(*args), name)
+
+
+def policy_layout(obs_dim, act_dim, hidden):
+    """(obs_cap, act_cap, hidden, P) of the zero-padded parameter layout of the *_padded policy entry points
+    (promp_policy_layout)."""
+    out = (c_int32 * 4)()
+    check(load().promp_policy_layout(int(obs_dim), int(act_dim), int(hidden), ctypes.cast(out, c_void_p)), 'promp_policy_layout')
+    return tuple(int(v) for v in out)

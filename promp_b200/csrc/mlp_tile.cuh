@@ -111,8 +111,10 @@ struct HeadIn {
     float c2[DA];      // 4 sig^2 / den^2
     float sum_ls;      // sum_d ls
 };
+// da: the logical action size; dimensions d >= da are the zero padding of a padded instantiation (DA = its cap) and are
+// left out of every sum, so that they contribute nothing and receive exactly zero gradient.
 template <int DA>
-__device__ __forceinline__ void head_in_finish(HeadIn<DA>& h) {
+__device__ __forceinline__ void head_in_finish(HeadIn<DA>& h, int da = DA) {
     h.sum_ls = 0.f;
 #pragma unroll
     for (int d = 0; d < DA; ++d) {
@@ -122,7 +124,7 @@ __device__ __forceinline__ void head_in_finish(HeadIn<DA>& h) {
         h.inv_den[d] = 1.f / den;
         h.c1[d] = 1.f - 2.f * h.s2[d] / den;
         h.c2[d] = 4.f * h.s2[d] / (den * den);
-        h.sum_ls += h.ls[d];
+        if (d < da) h.sum_ls += h.ls[d];
     }
 }
 // The old (sampling) distribution's log_std: per task when the phase stores one row per task, else per sample.
@@ -134,7 +136,7 @@ struct HeadOld {
     float sum_ls;
 };
 template <int DA>
-__device__ __forceinline__ void head_old_from(const float* ls_old, HeadOld<DA>& ho) {
+__device__ __forceinline__ void head_old_from(const float* ls_old, HeadOld<DA>& ho, int da = DA) {
     ho.sum_ls = 0.f;
 #pragma unroll
     for (int d = 0; d < DA; ++d) {
@@ -142,7 +144,7 @@ __device__ __forceinline__ void head_old_from(const float* ls_old, HeadOld<DA>& 
         ho.ls[d] = ls_old[d];
         ho.so2[d] = so * so;
         ho.inv_so[d] = 1.f / so;
-        ho.sum_ls += ls_old[d];
+        if (d < da) ho.sum_ls += ls_old[d];
     }
 }
 
@@ -161,10 +163,15 @@ constexpr float LOG_2PI = 1.8378770664093453f;
 
 template <int DA>
 __device__ __forceinline__ void gaussian_head(const HeadIn<DA>& hin, const HeadOld<DA>& ho, const float* mu, const float* a,
-                                              const float* mu_old, float adv, int obj_kind, float clip_eps, HeadOut<DA>& o) {
+                                              const float* mu_old, float adv, int obj_kind, float clip_eps, HeadOut<DA>& o,
+                                              int da = DA) {
     float sum_z2 = 0.f, sum_zo2 = 0.f, kl = 0.f;
 #pragma unroll
     for (int d = 0; d < DA; ++d) {
+        if (d >= da) {          // padding of a padded instantiation: no term, no gradient
+            o.zeta[d] = o.dkl_dmu[d] = o.dkl_dls[d] = 0.f;
+            continue;
+        }
         const float z = (a[d] - mu[d]) * hin.inv_sig[d];
         o.zeta[d] = z;
         sum_z2 += z * z;
@@ -177,8 +184,8 @@ __device__ __forceinline__ void gaussian_head(const HeadIn<DA>& hin, const HeadO
         o.dkl_dmu[d] = -2.f * dm * hin.inv_den[d];
         o.dkl_dls[d] = hin.c1[d] - hin.c2[d] * num;
     }
-    const float logp_new = -hin.sum_ls - 0.5f * sum_z2 - 0.5f * DA * LOG_2PI;   // log_likelihood_sym (:89-109)
-    const float logp_old = -ho.sum_ls - 0.5f * sum_zo2 - 0.5f * DA * LOG_2PI;
+    const float logp_new = -hin.sum_ls - 0.5f * sum_z2 - 0.5f * da * LOG_2PI;   // log_likelihood_sym (:89-109)
+    const float logp_old = -ho.sum_ls - 0.5f * sum_zo2 - 0.5f * da * LOG_2PI;
     const float ratio = expf(logp_new - logp_old);                           // likelihood_ratio_sym (:71-87)
     o.ratio = ratio;
     o.kl = kl;

@@ -9,6 +9,7 @@
 // crosses a task boundary (or ends) it flushes them to a per-(CTA,task) partial slot, and the last
 // segment of each task to arrive (atomic ticket) reduces that task's slots in CTA order -> bitwise
 // run-to-run deterministic sums.  These kernels are fp32-FMA bound (AI ~ 10^2..10^3 FLOP/B).
+#include <stddef.h>
 #include <string.h>
 #include "mlp_tile.cuh"
 
@@ -31,10 +32,14 @@ struct PolicyArgs {
     float obj_scale, clip_eps, kl_coeff;
     int clip_log_std;
     float min_log_std;
+    int obs_dim;         // logical observation / action sizes; read only by the padded instantiations (IsBucket below).  Both
+                         // sit in what was alignment padding: the struct's size and field offsets, and so the parameter
+                         // layout of every kernel taking PolicyArgs or ChainArgs, are unchanged.
     // grad kernel
     float* grad;
     float* out_params;
     float sgd_lr;
+    int act_dim;
     // hvp kernel
     const float* vec;
     float* out;
@@ -58,8 +63,32 @@ struct PolicyArgs {
     // iteration has no host decision: promp_adapt_kl_coeff updates it between launches)
     const float* kl_coeff_ptr;
 };
+static_assert(sizeof(PolicyArgs) == 224 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120,
+              "PolicyArgs layout");
 __device__ __forceinline__ float kl_coeff_eff(const PolicyArgs& A) {
     return A.kl_coeff_ptr ? A.kl_coeff * __ldcg(A.kl_coeff_ptr) : A.kl_coeff;
+}
+
+// Padded instantiations ("buckets"): compiled at the caps (DO, DA) of the zero-padded parameter layout of
+// promp_policy_layout, they take the logical observation / action sizes from PolicyArgs at run time.  Observations are
+// read with row stride obs_dim and zero-filled above it; action-side data (act, old_mean, old_log_std, mean) with row
+// stride act_dim, entries d >= act_dim never touched; the Gaussian head masks d >= act_dim out of every sum and gradient.
+// Pad rows of W0, pad columns of W2 and pad entries of b2 / log_std therefore get gradients and HVPs of exactly zero.
+// Whether a (DO, DA) instantiation is a bucket is known at compile time, so the exact instantiations compile to the code
+// they had.  The caps: obs_dim 1..8 -> 8, 9..19 -> 20; act_dim 1..2 -> 2, 3..8 -> 8 (even: P % 4 == 0).
+template <int DO, int DA>
+struct IsBucket {
+    static constexpr bool value = (DO == 8 || DO == 20) && (DA == 2 || DA == 8);
+};
+template <int DO, int DA>
+__device__ __forceinline__ int obs_dim_of(const PolicyArgs& A) {
+    if constexpr (IsBucket<DO, DA>::value) return A.obs_dim;
+    return DO;
+}
+template <int DO, int DA>
+__device__ __forceinline__ int act_dim_of(const PolicyArgs& A) {
+    if constexpr (IsBucket<DO, DA>::value) return A.act_dim;
+    return DA;
 }
 
 // consumer / producer halves of the launch re-use protocol above; returns true if the calling CTA must exit
@@ -120,17 +149,17 @@ __device__ __forceinline__ float4 reduce_segments4(const float* partial, const T
 }
 
 template <int DO, int DA, int HID>
-__device__ __forceinline__ void load_head_consts(const float* P, int clip, float min_ls, HeadIn<DA>& hin) {
+__device__ __forceinline__ void load_head_consts(const float* P, int clip, float min_ls, HeadIn<DA>& hin, int da = DA) {
     using L = PLayout<DO, DA, HID>;
 #pragma unroll
     for (int d = 0; d < DA; ++d) {
         const float raw = P[L::LS + d];
         const bool clipped = clip && (raw < min_ls);      // tf.maximum: gradient goes to x when x >= y
         hin.ls[d] = clipped ? min_ls : raw;
-        hin.ls_mask[d] = clipped ? 0.f : 1.f;
+        hin.ls_mask[d] = (clipped || d >= da) ? 0.f : 1.f;      // padding (d >= da) gets no log_std gradient either
         hin.sig[d] = expf(hin.ls[d]);
     }
-    head_in_finish<DA>(hin);
+    head_in_finish<DA>(hin, da);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -185,6 +214,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
     const int row0 = ty * RM, col0 = tx * 4;
     const int rb = tid >> 2, rq = tid & 3;           // row role
     const int cj = tid % HID, cp = tid / HID;        // column role
+    const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);
     if (grad_reuse_prologue<L::P, L::LS, DA>(A)) return;
     const TileSched ts(A.M, A.N, A.q);
     const int N = A.N;
@@ -224,7 +254,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
             const int j = i / HID, k = i % HID;      // consecutive threads -> consecutive W1T addresses
             S.W1T[j * HID + k] = S.P[L::W1 + k * HID + j];
         }
-        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin);
+        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin, dA);
     };
     // write this CTA's partial sums for task m; the last segment of the task reduces them in CTA order
     auto flush = [&](int m) {
@@ -329,7 +359,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
         __syncthreads();
         for (int i = tid; i < TB * DOP; i += PT_THREADS) {
             const int b = i / DOP, c = i % DOP;
-            S.X[i] = (b < nb && c < DO) ? __ldg(A.obs + (g0 + b) * DO + c) : 0.f;
+            S.X[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
         }
         __syncthreads();
         // ---- layer 0: H1 = tanh(X W0 + b0)                      (policies/networks/mlp.py:96-117)
@@ -389,15 +419,15 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
                     float a[DA], mo[DA], lso[DA];
 #pragma unroll
                     for (int d = 0; d < DA; ++d) {
-                        a[d] = __ldg(A.act + n * DA + d);
-                        mo[d] = __ldg(A.old_mean + n * DA + d);
-                        lso[d] = A.ls_per_sample ? __ldg(A.old_ls + n * DA + d) : __ldg(A.old_ls + (int64_t)m * DA + d);
+                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
+                        lso[d] = d >= dA ? 0.f : A.ls_per_sample ? __ldg(A.old_ls + n * dA + d) : __ldg(A.old_ls + (int64_t)m * dA + d);
                     }
                     const float adv = __ldg(A.adv + n);
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
-                    head_old_from<DA>(lso, ho);
-                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    head_old_from<DA>(lso, ho, dA);
+                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                     const float wt = A.obj_scale * o.w * invN, kc = kl_eff * invN;
 #pragma unroll
                     for (int d = 0; d < DA; ++d) {
@@ -530,6 +560,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
     const int row0 = ty * RM, col0 = tx * 4;
     const int rb = tid >> 2, rq = tid & 3;
     const int cj = tid % HID, cp = tid / HID;
+    const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);
     const TileSched ts(A.M, A.N, A.q);
     const int N = A.N;
     const float kl_eff = kl_coeff_eff(A);
@@ -574,7 +605,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             if (reload_p) S.W1T[j * HID + k] = S.P[L::W1 + k * HID + j];
             S.V1T[j * HID + k] = S.V[L::W1 + k * HID + j];
         }
-        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin);
+        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin, dA);
 #pragma unroll
         for (int d = 0; d < DA; ++d) rls[d] = S.V[L::LS + d] * hin.ls_mask[d];
     };
@@ -670,7 +701,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
         __syncthreads();
         for (int i = tid; i < TB * DOP; i += PT_THREADS) {
             const int b = i / DOP, c = i % DOP;
-            S.X[i] = (b < nb && c < DO) ? __ldg(A.obs + (g0 + b) * DO + c) : 0.f;
+            S.X[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
         }
         __syncthreads();
         // ---- layer 0 and its tangent: H1 = tanh(X W0 + b0); R1 = (1-H1^2) * (X V0 + vb0)
@@ -759,15 +790,15 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
                     float a[DA], mo[DA], lso[DA];
 #pragma unroll
                     for (int d = 0; d < DA; ++d) {
-                        a[d] = __ldg(A.act + n * DA + d);
-                        mo[d] = __ldg(A.old_mean + n * DA + d);
-                        lso[d] = A.ls_per_sample ? __ldg(A.old_ls + n * DA + d) : __ldg(A.old_ls + (int64_t)m * DA + d);
+                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
+                        lso[d] = d >= dA ? 0.f : A.ls_per_sample ? __ldg(A.old_ls + n * dA + d) : __ldg(A.old_ls + (int64_t)m * dA + d);
                     }
                     const float adv = __ldg(A.adv + n);
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
-                    head_old_from<DA>(lso, ho);
-                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    head_old_from<DA>(lso, ho, dA);
+                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                     const float wt = o.w * invN, kc = kl_eff * invN;
                     // tangent of log p:  R l = sum_d (zeta/sig) R mu + (zeta^2 - 1) R ls
                     float rl = 0.f;
@@ -785,6 +816,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
                         const float rdls = rwt * (z * z - 1.f) + wt * 2.f * z * rz;
                         cmu[d] = ac * rdmu + kc * o.dkl_dmu[d];
                         cls[d] = (ac * rdls + kc * o.dkl_dls[d]) * hin.ls_mask[d];
+                        if (d >= dA) dmu[d] = cmu[d] = 0.f;      // padding: exactly zero whatever the direction's pad entries hold
                     }
                     s_obj += o.obj;
                     s_kl += o.kl;
@@ -897,10 +929,11 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
 namespace promp {
 
 // -------------------------------------------------------------------------------------------------
-// forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling)
+// forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling).  dO / dA: the logical sizes
+// (= DO / DA for the exact instantiations, run-time values in policy_forward_padded_kernel)
 template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride,
-                                                              const float* obs, float* mean) {
+__device__ __forceinline__ void policy_forward_body(int M, int N, const float* params, int64_t stride, const float* obs,
+                                                    float* mean, int dO, int dA) {
     using L = PLayout<DO, DA, HID>;
     constexpr int NU = HID / 32;
     __shared__ float sP[L::P];
@@ -910,12 +943,12 @@ __global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const
     for (int i = threadIdx.x; i < L::P; i += blockDim.x) sP[i] = __ldg(th + i);
     __syncthreads();
     for (int n = blockIdx.x * 4 + w; n < N; n += gridDim.x * 4) {
-        const float* o = obs + ((int64_t)m * N + n) * DO;
+        const float* o = obs + ((int64_t)m * N + n) * dO;
 #pragma unroll
         for (int u = 0; u < NU; ++u) {
             const int j = lane + 32 * u;
             float z = sP[L::B0 + j];
-            for (int i = 0; i < DO; ++i) z = fmaf(__ldg(o + i), sP[L::W0 + i * HID + j], z);
+            for (int i = 0; i < dO; ++i) z = fmaf(__ldg(o + i), sP[L::W0 + i * HID + j], z);
             sh[w][j] = tanh_fast(z);
         }
         __syncwarp();
@@ -934,10 +967,20 @@ __global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const
 #pragma unroll
         for (int d = 0; d < DA; ++d) {
             const float s = warp_sum(mu[d]) + sP[L::B2 + d];
-            if (lane == d) mean[((int64_t)m * N + n) * DA + d] = s;
+            if (lane == d && d < dA) mean[((int64_t)m * N + n) * dA + d] = s;
         }
         __syncwarp();
     }
+}
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride,
+                                                              const float* obs, float* mean) {
+    policy_forward_body<DO, DA, HID>(M, N, params, stride, obs, mean, DO, DA);
+}
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(128) policy_forward_padded_kernel(int M, int N, const float* params, int64_t stride,
+                                                                     const float* obs, float* mean, int obs_dim, int act_dim) {
+    policy_forward_body<DO, DA, HID>(M, N, params, stride, obs, mean, obs_dim, act_dim);
 }
 
 __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, float* out) {
@@ -1339,14 +1382,19 @@ static int64_t chain_ws_bytes(int n_stages, const int* kinds, const int* Ns, int
 }
 
 template <int DO, int DA, int HID>
-static int launch_forward(int M, int N, const float* params, int64_t stride, const float* obs, float* mean,
-                          cudaStream_t st) {
+static int launch_forward(int M, int N, const float* params, int64_t stride, const float* obs, float* mean, int obs_dim,
+                          int act_dim, cudaStream_t st) {
     int gx = (N + 3) / 4;
     const int cap = (4 * sm_count() + M - 1) / M;
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    policy_forward_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean);
-    PROMP_LAUNCH_CHECK("policy_forward_kernel");
+    if constexpr (IsBucket<DO, DA>::value) {
+        policy_forward_padded_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+        PROMP_LAUNCH_CHECK("policy_forward_padded_kernel");
+    } else {
+        policy_forward_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean);
+        PROMP_LAUNCH_CHECK("policy_forward_kernel");
+    }
     return PROMP_OK;
 }
 
@@ -1361,6 +1409,23 @@ static int launch_forward(int M, int N, const float* params, int64_t stride, con
     set_error("unsupported (obs_dim, act_dim, hidden) = (%d, %d, %d); built: (2,2,{32,64}), (4,2,{32,64}), (17,6,{32,64})", \
               obs_dim, act_dim, hidden);                                                       \
     return PROMP_ERR_INVALID_ARG;
+
+// the padded (bucket) instantiations, at the caps promp_policy_layout gives (obs, act, hidden)
+#define PROMP_DISPATCH_BUCKETS(FN, ...)                                                                      \
+    {                                                                                                        \
+        int32_t lay_[4];                                                                                     \
+        if (promp_policy_layout(obs_dim, act_dim, hidden, lay_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;  \
+        if (lay_[0] == 8 && lay_[1] == 2 && hidden == 64) return FN<8, 2, 64>(__VA_ARGS__);                 \
+        if (lay_[0] == 8 && lay_[1] == 2 && hidden == 32) return FN<8, 2, 32>(__VA_ARGS__);                 \
+        if (lay_[0] == 8 && lay_[1] == 8 && hidden == 64) return FN<8, 8, 64>(__VA_ARGS__);                 \
+        if (lay_[0] == 8 && lay_[1] == 8 && hidden == 32) return FN<8, 8, 32>(__VA_ARGS__);                 \
+        if (lay_[0] == 20 && lay_[1] == 2 && hidden == 64) return FN<20, 2, 64>(__VA_ARGS__);               \
+        if (lay_[0] == 20 && lay_[1] == 2 && hidden == 32) return FN<20, 2, 32>(__VA_ARGS__);               \
+        if (lay_[0] == 20 && lay_[1] == 8 && hidden == 64) return FN<20, 8, 64>(__VA_ARGS__);               \
+        if (lay_[0] == 20 && lay_[1] == 8 && hidden == 32) return FN<20, 8, 32>(__VA_ARGS__);               \
+        set_error("no padded instantiation for caps (%d, %d, %d)", lay_[0], lay_[1], hidden);               \
+        return PROMP_ERR_INVALID_ARG;                                                                        \
+    }
 
 }  // namespace promp
 
@@ -1380,6 +1445,24 @@ extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int a
     return counters_bytes(M) + worst * (int64_t)sizeof(float) + 16;
 }
 
+extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]) {
+    PROMP_REQUIRE(out != nullptr, "promp_policy_layout: null output");
+    PROMP_REQUIRE(obs_dim >= 1 && obs_dim <= 19 && act_dim >= 1 && act_dim <= 8 && (hidden == 32 || hidden == 64),
+                  "promp_policy_layout: padded policy kernels take obs_dim in [1, 19], act_dim in [1, 8] and hidden 32 or 64 "
+                  "(got %d, %d, %d)", obs_dim, act_dim, hidden);
+    out[0] = obs_dim <= 8 ? 8 : 20;
+    out[1] = act_dim <= 2 ? 2 : 8;
+    out[2] = hidden;
+    out[3] = promp::num_params(out[0], out[1], hidden);
+    return PROMP_OK;
+}
+
+extern "C" int64_t promp_policy_workspace_bytes_padded(int M, int N, int obs_dim, int act_dim, int hidden) {
+    int32_t lay[4];
+    if (promp_policy_layout(obs_dim, act_dim, hidden, lay) != PROMP_OK) return -1;
+    return promp_policy_workspace_bytes(M, N, lay[0], lay[1], hidden);
+}
+
 static int check_policy_args(const char* who, int M, int N, const void* params, const void* obs, const void* act,
                              const void* adv, const void* old_mean, const void* old_ls, const void* ws) {
     PROMP_REQUIRE(M > 0 && N > 0, "%s: M and N must be positive (got %d, %d)", who, M, N);
@@ -1387,13 +1470,14 @@ static int check_policy_args(const char* who, int M, int N, const void* params, 
     return PROMP_OK;
 }
 
-extern "C" int promp_policy_grad_ex(int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
-                                    const float* params, int64_t param_stride, const float* obs, const float* act,
-                                    const float* adv, const float* old_mean, const float* old_log_std, int ls_per_sample,
-                                    int obj_kind, float obj_scale, float clip_eps, float kl_coeff, int clip_log_std,
-                                    float min_log_std, float* grad, float* out_params, float sgd_lr, float* stats,
-                                    const int32_t* skip_flag, const float* skip_theta, int32_t* unclipped_out, float* theta_copy_out,
-                                    void* workspace, int64_t workspace_bytes, void* stream) {
+// padded: the bucket instantiations (promp_*_padded entry points), else the exact table
+static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
+                            const float* params, int64_t param_stride, const float* obs, const float* act,
+                            const float* adv, const float* old_mean, const float* old_log_std, int ls_per_sample,
+                            int obj_kind, float obj_scale, float clip_eps, float kl_coeff, int clip_log_std,
+                            float min_log_std, float* grad, float* out_params, float sgd_lr, float* stats,
+                            const int32_t* skip_flag, const float* skip_theta, int32_t* unclipped_out, float* theta_copy_out,
+                            void* workspace, int64_t workspace_bytes, void* stream) {
     int st = check_policy_args(n_valid ? "promp_policy_grad_ragged" : "promp_policy_grad", M, N, params, obs, act, adv, old_mean, old_log_std, workspace);
     if (st != PROMP_OK) return st;
     PROMP_REQUIRE(obj_kind >= 0 && obj_kind <= 3, "promp_policy_grad: bad obj_kind %d", obj_kind);
@@ -1409,9 +1493,25 @@ extern "C" int promp_policy_grad_ex(int obs_dim, int act_dim, int hidden, int M,
     A.kl_coeff = kl_coeff; A.clip_log_std = clip_log_std; A.min_log_std = min_log_std;
     A.grad = grad; A.out_params = out_params; A.sgd_lr = sgd_lr; A.stats = stats; A.n_valid = n_valid;
     A.skip_flag = skip_flag; A.skip_theta = skip_theta; A.unclipped_out = unclipped_out; A.theta_copy_out = theta_copy_out;
+    A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
+    if (padded) PROMP_DISPATCH_BUCKETS(launch_grad_any, A, workspace, workspace_bytes, s)
     PROMP_DISPATCH_DIMS(launch_grad_any, A, workspace, workspace_bytes, s)
 }
+
+#define PROMP_GRAD_EX_PARAMS                                                                                               \
+    int obs_dim, int act_dim, int hidden, int M, int N, const int32_t *n_valid, const float *params, int64_t param_stride, \
+        const float *obs, const float *act, const float *adv, const float *old_mean, const float *old_log_std,             \
+        int ls_per_sample, int obj_kind, float obj_scale, float clip_eps, float kl_coeff, int clip_log_std,                \
+        float min_log_std, float *grad, float *out_params, float sgd_lr, float *stats, const int32_t *skip_flag,           \
+        const float *skip_theta, int32_t *unclipped_out, float *theta_copy_out, void *workspace, int64_t workspace_bytes,  \
+        void *stream
+#define PROMP_GRAD_EX_ARGS                                                                                                 \
+    obs_dim, act_dim, hidden, M, N, n_valid, params, param_stride, obs, act, adv, old_mean, old_log_std, ls_per_sample,    \
+        obj_kind, obj_scale, clip_eps, kl_coeff, clip_log_std, min_log_std, grad, out_params, sgd_lr, stats, skip_flag,    \
+        skip_theta, unclipped_out, theta_copy_out, workspace, workspace_bytes, stream
+extern "C" int promp_policy_grad_ex(PROMP_GRAD_EX_PARAMS) { return policy_grad_impl(false, PROMP_GRAD_EX_ARGS); }
+extern "C" int promp_policy_grad_ex_padded(PROMP_GRAD_EX_PARAMS) { return policy_grad_impl(true, PROMP_GRAD_EX_ARGS); }
 
 extern "C" int promp_policy_grad_ragged(int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
                                         const float* params, int64_t param_stride, const float* obs, const float* act,
@@ -1435,12 +1535,12 @@ extern "C" int promp_policy_grad(int obs_dim, int act_dim, int hidden, int M, in
                                     grad, out_params, sgd_lr, stats, workspace, workspace_bytes, stream);
 }
 
-extern "C" int promp_policy_hvp_ragged(int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
-                                       const float* params, int64_t param_stride, const float* obs, const float* act,
-                                       const float* adv, const float* old_mean, const float* old_log_std, int ls_per_sample,
-                                       int obj_kind, float inner_lr, float kl_coeff, int clip_log_std, float min_log_std,
-                                       const float* vec, float* out, float* stats, void* workspace, int64_t workspace_bytes,
-                                       void* stream) {
+static int policy_hvp_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
+                           const float* params, int64_t param_stride, const float* obs, const float* act,
+                           const float* adv, const float* old_mean, const float* old_log_std, int ls_per_sample,
+                           int obj_kind, float inner_lr, float kl_coeff, int clip_log_std, float min_log_std,
+                           const float* vec, float* out, float* stats, void* workspace, int64_t workspace_bytes,
+                           void* stream) {
     int st = check_policy_args(n_valid ? "promp_policy_hvp_ragged" : "promp_policy_hvp", M, N, params, obs, act, adv, old_mean, old_log_std, workspace);
     if (st != PROMP_OK) return st;
     PROMP_REQUIRE(obj_kind == PROMP_OBJ_RATIO || obj_kind == PROMP_OBJ_LOGLIK,
@@ -1452,9 +1552,22 @@ extern "C" int promp_policy_hvp_ragged(int obs_dim, int act_dim, int hidden, int
     A.ls_per_sample = ls_per_sample; A.obj_kind = obj_kind; A.obj_scale = 1.f; A.clip_eps = 0.f;
     A.kl_coeff = kl_coeff; A.clip_log_std = clip_log_std; A.min_log_std = min_log_std;
     A.vec = vec; A.out = out; A.inner_lr = inner_lr; A.stats = stats; A.n_valid = n_valid;
+    A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
+    if (padded) PROMP_DISPATCH_BUCKETS(launch_hvp, A, workspace, workspace_bytes, s)
     PROMP_DISPATCH_DIMS(launch_hvp, A, workspace, workspace_bytes, s)
 }
+
+#define PROMP_HVP_RAGGED_PARAMS                                                                                            \
+    int obs_dim, int act_dim, int hidden, int M, int N, const int32_t *n_valid, const float *params, int64_t param_stride, \
+        const float *obs, const float *act, const float *adv, const float *old_mean, const float *old_log_std,             \
+        int ls_per_sample, int obj_kind, float inner_lr, float kl_coeff, int clip_log_std, float min_log_std,              \
+        const float *vec, float *out, float *stats, void *workspace, int64_t workspace_bytes, void *stream
+#define PROMP_HVP_RAGGED_ARGS                                                                                              \
+    obs_dim, act_dim, hidden, M, N, n_valid, params, param_stride, obs, act, adv, old_mean, old_log_std, ls_per_sample,    \
+        obj_kind, inner_lr, kl_coeff, clip_log_std, min_log_std, vec, out, stats, workspace, workspace_bytes, stream
+extern "C" int promp_policy_hvp_ragged(PROMP_HVP_RAGGED_PARAMS) { return policy_hvp_impl(false, PROMP_HVP_RAGGED_ARGS); }
+extern "C" int promp_policy_hvp_ragged_padded(PROMP_HVP_RAGGED_PARAMS) { return policy_hvp_impl(true, PROMP_HVP_RAGGED_ARGS); }
 
 extern "C" int promp_policy_hvp(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
                                 int64_t param_stride, const float* obs, const float* act, const float* adv,
@@ -1497,25 +1610,43 @@ static int chain_stage_args(const promp_policy_stage* stages, int n_stages, int 
     return PROMP_OK;
 }
 
-extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
-                                                      const promp_policy_stage* stages) {
+static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                                 const promp_policy_stage* stages) {
     if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
+    if (padded) PROMP_DISPATCH_BUCKETS(chain_ws_bytes, n_stages, kinds, Ns, M)
     PROMP_DISPATCH_DIMS(chain_ws_bytes, n_stages, kinds, Ns, M)
 }
+extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                                      const promp_policy_stage* stages) {
+    return policy_chain_workspace_bytes_impl(false, obs_dim, act_dim, hidden, M, n_stages, stages);
+}
+extern "C" int64_t promp_policy_chain_workspace_bytes_padded(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                                             const promp_policy_stage* stages) {
+    return policy_chain_workspace_bytes_impl(true, obs_dim, act_dim, hidden, M, n_stages, stages);
+}
 
-extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
-                                               const promp_policy_stage* stages) {
+static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                          const promp_policy_stage* stages) {
     if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
+    if (padded) PROMP_DISPATCH_BUCKETS(chain_num_launches, n_stages, kinds, Ns, M)
     PROMP_DISPATCH_DIMS(chain_num_launches, n_stages, kinds, Ns, M)
 }
+extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                               const promp_policy_stage* stages) {
+    return policy_chain_num_launches_impl(false, obs_dim, act_dim, hidden, M, n_stages, stages);
+}
+extern "C" int promp_policy_chain_num_launches_padded(int obs_dim, int act_dim, int hidden, int M, int n_stages,
+                                                      const promp_policy_stage* stages) {
+    return policy_chain_num_launches_impl(true, obs_dim, act_dim, hidden, M, n_stages, stages);
+}
 
-extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
-                                  const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
-                                  void* workspace, int64_t workspace_bytes, void* stream) {
+static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
+                             const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
+                             void* workspace, int64_t workspace_bytes, void* stream) {
     PROMP_REQUIRE(M > 0 && workspace != nullptr, "promp_policy_chain: M must be positive and workspace non-null");
     PROMP_REQUIRE((skip_flag == nullptr) == (skip_theta == nullptr), "promp_policy_chain: skip_flag / skip_theta come as a pair");
     PolicyArgs A[CHAIN_MAX_STAGES];
@@ -1524,8 +1655,22 @@ extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, f
     if (rc != PROMP_OK) return rc;
     PROMP_REQUIRE(!skip_flag || (kinds[0] == 0 && A[0].param_stride == 0),
                   "promp_policy_chain: launch re-use is defined for a gradient stage 0 on shared parameters (param_stride 0)");
+    for (int k = 0; k < n_stages; ++k) A[k].obs_dim = obs_dim, A[k].act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
+    if (padded) PROMP_DISPATCH_BUCKETS(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, workspace, workspace_bytes, s)
     PROMP_DISPATCH_DIMS(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, workspace, workspace_bytes, s)
+}
+extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
+                                  const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
+                                  void* workspace, int64_t workspace_bytes, void* stream) {
+    return policy_chain_impl(false, obs_dim, act_dim, hidden, M, min_log_std, n_stages, stages, skip_flag, skip_theta, workspace,
+                             workspace_bytes, stream);
+}
+extern "C" int promp_policy_chain_padded(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
+                                         const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+    return policy_chain_impl(true, obs_dim, act_dim, hidden, M, min_log_std, n_stages, stages, skip_flag, skip_theta, workspace,
+                             workspace_bytes, stream);
 }
 
 extern "C" int promp_set_option(const char* name, int value) {
@@ -1556,12 +1701,21 @@ extern "C" int promp_set_option(const char* name, int value) {
     return PROMP_ERR_INVALID_ARG;
 }
 
-extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
-                                    int64_t param_stride, const float* obs, float* mean, void* stream) {
+static int policy_forward_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
+                               int64_t param_stride, const float* obs, float* mean, void* stream) {
     PROMP_REQUIRE(M > 0 && N > 0 && params && obs && mean, "promp_policy_forward: bad arguments");
     PROMP_REQUIRE(M <= 65535, "promp_policy_forward: M=%d exceeds the grid.y limit", M);
     cudaStream_t s = (cudaStream_t)stream;
-    PROMP_DISPATCH_DIMS(launch_forward, M, N, params, param_stride, obs, mean, s)
+    if (padded) PROMP_DISPATCH_BUCKETS(launch_forward, M, N, params, param_stride, obs, mean, obs_dim, act_dim, s)
+    PROMP_DISPATCH_DIMS(launch_forward, M, N, params, param_stride, obs, mean, obs_dim, act_dim, s)
+}
+extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
+                                    int64_t param_stride, const float* obs, float* mean, void* stream) {
+    return policy_forward_impl(false, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, stream);
+}
+extern "C" int promp_policy_forward_padded(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
+                                           int64_t param_stride, const float* obs, float* mean, void* stream) {
+    return policy_forward_impl(true, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, stream);
 }
 
 extern "C" int promp_reduce_tasks(int M, int P, const float* in, float scale, float* out, void* stream) {

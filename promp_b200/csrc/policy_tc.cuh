@@ -364,6 +364,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
     const int qd = warp & 3, cq = warp >> 2;               // row quadrant, column group
     const int r = qd * 32 + lane, c0 = CW * cq;          // row / column-group role: sample row r, hidden units [c0, c0+32)
     const int cj = tid & (HID - 1), cp = tid / HID;        // column role
+    const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);      // logical sizes (padded instantiations)
     const int N = A.N;
     const float kl_eff = kl_coeff_eff(A);      // kl_coeff, times the device-resident multiplier when there is one
     float invN = 1.0f / (float)N;       // both re-set per task when A.n_valid is given (variable-length paths)
@@ -424,15 +425,15 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                 const float raw = S.Ps[SL::LS + d];
                 const bool clipped = A.clip_log_std && (raw < A.min_log_std);
                 hin.ls[d] = clipped ? A.min_log_std : raw;
-                hin.ls_mask[d] = clipped ? 0.f : 1.f;
+                hin.ls_mask[d] = (clipped || d >= dA) ? 0.f : 1.f;
                 hin.sig[d] = expf(hin.ls[d]);
             }
-            head_in_finish<DA>(hin);
+            head_in_finish<DA>(hin, dA);
             if (!A.ls_per_sample) {
                 float lso[DA];
 #pragma unroll
-                for (int d = 0; d < DA; ++d) lso[d] = __ldg(A.old_ls + (int64_t)m * DA + d);
-                head_old_from<DA>(lso, S.hold);
+                for (int d = 0; d < DA; ++d) lso[d] = d < dA ? __ldg(A.old_ls + (int64_t)m * dA + d) : 0.f;
+                head_old_from<DA>(lso, S.hold, dA);
             }
         }
         __syncthreads();
@@ -559,7 +560,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #pragma unroll
         for (int e = 0; e < (XPRE ? XR : 1); ++e) {
             const int i = tid + e * TCT, b = i / DOP, c = i % DOP;
-            dst[e] = (b < nb_ && c < DO) ? __ldg(A.obs + ((int64_t)m_ * N + n0_ + b) * DO + c) : 0.f;
+            dst[e] = (b < nb_ && c < dO) ? __ldg(A.obs + ((int64_t)m_ * N + n0_ + b) * dO + c) : 0.f;
         }
     };
     int cur_m = -1;
@@ -589,16 +590,16 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                 const int64_t n = g0 + r;
 #pragma unroll
                 for (int d = 0; d < DA; ++d) {
-                    ha[d] = __ldg(A.act + n * DA + d);
-                    hmo[d] = __ldg(A.old_mean + n * DA + d);
-                    if (A.ls_per_sample) hlso[d] = __ldg(A.old_ls + n * DA + d);
+                    ha[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                    hmo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
+                    if (A.ls_per_sample) hlso[d] = d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
                 }
                 hadv = __ldg(A.adv + n);
             }
         } else {
             for (int i = tid; i < TBT * DOP; i += TCT) {
                 const int b = i / DOP, c = i % DOP;
-                S.X[i] = (b < nb && c < DO) ? __ldg(A.obs + (g0 + b) * DO + c) : 0.f;
+                S.X[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
             }
         }
         __syncthreads();
@@ -669,8 +670,8 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     if constexpr (XPRE) {
                         a[d] = ha[d], mo[d] = hmo[d];
                     } else {
-                        a[d] = __ldg(A.act + n * DA + d);
-                        mo[d] = __ldg(A.old_mean + n * DA + d);
+                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
                     }
                 }
                 const float adv = XPRE ? hadv : __ldg(A.adv + n);
@@ -679,11 +680,11 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     float lso[DA];
                     HeadOld<DA> ho;
 #pragma unroll
-                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : __ldg(A.old_ls + n * DA + d);
-                    head_old_from<DA>(lso, ho);
-                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
+                    head_old_from<DA>(lso, ho, dA);
+                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 } else {
-                    gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
                 const float wt = A.obj_scale * o.w * invN, kc = kl_eff * invN;
 #pragma unroll
@@ -858,6 +859,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
     const int qd = warp & 3, cq = warp >> 2;               // row quadrant, column group
     const int r = qd * 32 + lane, c0 = CW * cq;
     const int cj = tid & (HID - 1), cp = tid / HID;
+    const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);
     const int N = A.N;
     const float kl_eff = kl_coeff_eff(A);      // kl_coeff, times the device-resident multiplier when there is one
     float invN = 1.0f / (float)N;       // both re-set per task when A.n_valid is given (variable-length paths)
@@ -914,15 +916,15 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                 const float raw = S.Ps[SL::LS + d];
                 const bool clipped = A.clip_log_std && (raw < A.min_log_std);
                 hin.ls[d] = clipped ? A.min_log_std : raw;
-                hin.ls_mask[d] = clipped ? 0.f : 1.f;
+                hin.ls_mask[d] = (clipped || d >= dA) ? 0.f : 1.f;
                 hin.sig[d] = expf(hin.ls[d]);
             }
-            head_in_finish<DA>(hin);
+            head_in_finish<DA>(hin, dA);
             if (!A.ls_per_sample) {
                 float lso[DA];
 #pragma unroll
-                for (int d = 0; d < DA; ++d) lso[d] = __ldg(A.old_ls + (int64_t)m * DA + d);
-                head_old_from<DA>(lso, S.hold);
+                for (int d = 0; d < DA; ++d) lso[d] = d < dA ? __ldg(A.old_ls + (int64_t)m * dA + d) : 0.f;
+                head_old_from<DA>(lso, S.hold, dA);
             }
         }
         __syncthreads();
@@ -1064,7 +1066,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
 #pragma unroll
         for (int e = 0; e < (XPRE ? XR : 1); ++e) {
             const int i = tid + e * TCT, b = i / DOP, c = i % DOP;
-            dst[e] = (b < nb_ && c < DO) ? __ldg(A.obs + ((int64_t)m_ * N + n0_ + b) * DO + c) : 0.f;
+            dst[e] = (b < nb_ && c < dO) ? __ldg(A.obs + ((int64_t)m_ * N + n0_ + b) * dO + c) : 0.f;
         }
     };
     int cur_m = -1;
@@ -1083,7 +1085,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
         auto load_x = [&]() {
             for (int i = tid; i < TBT * DOP; i += TCT) {
                 const int b = i / DOP, c = i % DOP;
-                sX[i] = (b < nb && c < DO) ? __ldg(A.obs + (g0 + b) * DO + c) : 0.f;
+                sX[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
             }
         };
         if constexpr (XPRE) {      // software pipeline, as in grad_tc_tiles; xc keeps this tile's elements for the second use below
@@ -1095,9 +1097,9 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                 const int64_t n = g0 + r;
 #pragma unroll
                 for (int d = 0; d < DA; ++d) {
-                    ha[d] = __ldg(A.act + n * DA + d);
-                    hmo[d] = __ldg(A.old_mean + n * DA + d);
-                    if (A.ls_per_sample) hlso[d] = __ldg(A.old_ls + n * DA + d);
+                    ha[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                    hmo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
+                    if (A.ls_per_sample) hlso[d] = d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
                 }
                 hadv = __ldg(A.adv + n);
             }
@@ -1192,8 +1194,8 @@ float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
                     if constexpr (XPRE) {
                         a[d] = ha[d], mo[d] = hmo[d];
                     } else {
-                        a[d] = __ldg(A.act + n * DA + d);
-                        mo[d] = __ldg(A.old_mean + n * DA + d);
+                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
+                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
                     }
                 }
                 const float adv = XPRE ? hadv : __ldg(A.adv + n);
@@ -1202,11 +1204,11 @@ float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
                     float lso[DA];
                     HeadOld<DA> ho;
 #pragma unroll
-                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : __ldg(A.old_ls + n * DA + d);
-                    head_old_from<DA>(lso, ho);
-                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
+                    head_old_from<DA>(lso, ho, dA);
+                    gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 } else {
-                    gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o);
+                    gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
                 const float wt = o.w * invN, kc = kl_eff * invN;
                 float rl_ = 0.f;
@@ -1223,6 +1225,7 @@ float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
                     const float rdls = rwt * (z * z - 1.f) + wt * 2.f * z * rz;
                     cmu[d] = ac * rdmu + kc * o.dkl_dmu[d];
                     cls[d] = (ac * rdls + kc * o.dkl_dls[d]) * hin.ls_mask[d];
+                    if (d >= dA) dmu[d] = cmu[d] = 0.f;      // padding: exactly zero whatever the direction's pad entries hold
                 }
                 s_obj += o.obj;
                 s_kl += o.kl;

@@ -19,6 +19,11 @@ PARAM_NAMES = ('mean_network/hidden_0/kernel', 'mean_network/hidden_0/bias',
                'mean_network/hidden_1/kernel', 'mean_network/hidden_1/bias',
                'mean_network/output/kernel', 'mean_network/output/bias',
                'log_std_network/log_std_var')
+# (obs_dim, action_dim) with policy kernels of their own; every other shape in range runs on the zero-padded kernels
+EXACT_SHAPES = ((2, 2), (4, 2), (17, 6))
+MAX_OBS_DIM, MAX_ACTION_DIM = 19, 8
+# C entry points the algorithms call, by role; a padded shape uses the *_padded sibling of each
+POLICY_ENTRIES = ('workspace_bytes', 'forward', 'grad_ex', 'hvp_ragged', 'chain', 'chain_workspace_bytes', 'chain_num_launches')
 
 
 def _is_tanh(fn):
@@ -35,6 +40,9 @@ class MetaGaussianMLPPolicy(object):
         if len(hidden_sizes) != 2 or max(hidden_sizes) > 64 or min(hidden_sizes) < 1:
             raise NotImplementedError("promp_b200 kernels are built for two tanh hidden layers of up to 64 units each "
                                       "(got hidden_sizes=%r)" % (hidden_sizes,))
+        if not (1 <= int(obs_dim) <= MAX_OBS_DIM and 1 <= int(action_dim) <= MAX_ACTION_DIM):
+            raise NotImplementedError("promp_b200 policy kernels take obs_dim in [1, %d] and action_dim in [1, %d] (got %d, %d)"
+                                      % (MAX_OBS_DIM, MAX_ACTION_DIM, int(obs_dim), int(action_dim)))
         if not _is_tanh(hidden_nonlinearity) or output_nonlinearity is not None:
             raise NotImplementedError("promp_b200 kernels implement tanh hidden / identity output non-linearities")
         if not learn_std:
@@ -58,10 +66,17 @@ class MetaGaussianMLPPolicy(object):
         self.param_shapes = OrderedDict(zip(PARAM_NAMES, (
             (self.obs_dim, h0), (h0,), (h0, h1), (h1,), (h1, self.action_dim), (self.action_dim,), (1, self.action_dim))))
         self.num_params_logical = int(sum(np.prod(sh) for sh in self.param_shapes.values()))
-        dev_shapes = ((self.obs_dim, Hd), (Hd,), (Hd, Hd), (Hd,), (Hd, self.action_dim), (self.action_dim,),
-                      (1, self.action_dim))
+        # Shapes outside EXACT_SHAPES pad the observation and action axes the same way: W0 gets zero rows up to obs_cap,
+        # W2 / b2 / log_std zero columns up to act_cap (promp_policy_layout), and the padded kernels keep them at zero.
+        self.padded_dims = (self.obs_dim, self.action_dim) not in EXACT_SHAPES
+        if self.padded_dims:
+            do_cap, da_cap, _, _ = _lib.policy_layout(self.obs_dim, self.action_dim, Hd)
+        else:
+            do_cap, da_cap = self.obs_dim, self.action_dim
+        self.entries = {k: 'promp_policy_' + k + ('_padded' if self.padded_dims else '') for k in POLICY_ENTRIES}
+        dev_shapes = ((do_cap, Hd), (Hd,), (Hd, Hd), (Hd,), (Hd, da_cap), (da_cap,), (1, da_cap))
         self.num_params = int(sum(np.prod(sh) for sh in dev_shapes))          # device (padded) vector length
-        assert self.num_params == _lib.load().promp_num_params(self.obs_dim, self.action_dim, self.hidden)
+        assert self.num_params == _lib.load().promp_num_params(do_cap, da_cap, self.hidden)
         # positions of the logical parameters inside the padded device vector
         idx, off = [], 0
         for (key, shape), dshape in zip(self.param_shapes.items(), dev_shapes):
@@ -69,6 +84,7 @@ class MetaGaussianMLPPolicy(object):
             idx.append(grid[tuple(slice(0, n) for n in shape)].reshape(-1))
             off += int(np.prod(dshape))
         self._pad_index_np = np.concatenate(idx)
+        self._log_std_lo = self.num_params - da_cap        # the logical log_std: [lo, lo + action_dim) of the device vector
         self.policy_params_keys = list(PARAM_NAMES)
         # Xavier-uniform kernels, zero biases, log_std = log(init_std)
         # (policies/networks/mlp.py:12-13, gaussian_mlp_policy.py:64-69); drawn from the numpy global RNG
@@ -188,10 +204,10 @@ class MetaGaussianMLPPolicy(object):
         assert obs.shape[2] == self.obs_dim
         params, stride, clip = self.sampling_params()
         mean = torch.empty(M, E, self.action_dim, dtype=torch.float32, device=self.device)
-        _lib.call('promp_policy_forward', self.obs_dim, self.action_dim, self.hidden, M, E, _lib.ptr(params), stride,
+        _lib.call(self.entries['forward'], self.obs_dim, self.action_dim, self.hidden, M, E, _lib.ptr(params), stride,
                   _lib.ptr(obs.contiguous()), _lib.ptr(mean), _lib.stream())
         pm = params.view(-1, self.num_params) if stride else params.view(1, -1).expand(M, -1)
-        ls = pm[:, -self.action_dim:]
+        ls = pm[:, self._log_std_lo:self._log_std_lo + self.action_dim]
         actions = mean + torch.randn_like(mean) * torch.exp(ls).unsqueeze(1)
         rep = torch.clamp(ls, min=self.min_log_std) if clip else ls
         a, mu, rep = actions.cpu().numpy(), mean.cpu().numpy(), rep.cpu().numpy()
