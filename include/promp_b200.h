@@ -473,7 +473,7 @@ int promp_allreduce_p2p(int world, int rank, int n, int capacity_floats, const f
 
 /* Runtime options.
  *   "tensor_cores" = 1 (default): hidden-64 promp_policy_grad / promp_policy_hvp run their layer and weight-gradient GEMMs on
- *                    the tensor cores (mma.sync tf32, 3xTF32 split), same results to fp32 round-off; 0 = CUDA cores.
+ *                    the tensor cores (wgmma / mma.sync tf32, 3xTF32 split), same results to fp32 round-off; 0 = CUDA cores.
  *   "tc_threads"   = 0 (default: 512 threads per CTA for obs_dim <= 4, else 256), or force 256 / 512. */
 int promp_set_option(const char* name, int value);
 

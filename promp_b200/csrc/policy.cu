@@ -1117,7 +1117,7 @@ __global__ void adapt_kl_coeff_kernel(int S1, const float* __restrict__ final_te
 }
 
 // -------------------------------------------------------------------------------------------------
-static int g_use_tc = 1;     // promp_set_option("tensor_cores", 0|1): HID = 64 policy kernels on mma.sync 3xTF32 (default) or CUDA cores
+static int g_use_tc = 1;     // promp_set_option("tensor_cores", 0|1): HID = 64 policy kernels on the tensor cores, 3xTF32 (default) or CUDA cores
 
 static int g_tc_threads = 0;  // promp_set_option("tc_threads", 0|256|512): 0 = per-shape default
 // column groups of the TC kernels' thread mapping: 2 -> 256 threads (32 hidden units per thread), 4 -> 512 threads (16)

@@ -1,18 +1,19 @@
 // Tensor-core variant of policy_grad_kernel for HID = 64.
 //
 // The two [128 x 64] x [64 x 64] layer GEMMs of a tile (forward H1.W1 and backward D2.W1^T) run on the tensor cores as
-// warp-level mma.sync m16n8k8 tf32 with the 3-term split  a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  (a_hi =
+// warpgroup MMAs (wgmma.mma_async m64nNk8 tf32) with the 3-term split  a*b ~= a_hi*b_hi + a_lo*b_hi + a_hi*b_lo  (a_hi =
 // trunc_tf32(a), a_lo = a - a_hi), i.e. fp32-level accuracy at 3 MMAs per product.  Every warp of the CTA takes part:
 // warp w computes rows [16 (w % 8), +16) and 64 / (NW / 8) of the 64 output columns, accumulating in registers.  The A
-// operand (activations) is split into hi / lo while its fragments are loaded; the B operand (weights) is stored once per
-// task as hi + lo tiles.  Activation and weight tiles sit in shared memory in a K-major core-matrix layout: 8x4-float core
-// matrices (128 contiguous bytes, rows 16 B apart), next 8 rows at +128 B, next 4 columns at +S_c.  S_c = rows*16 + 16
-// bytes: the extra 16 B make the row-wise 16-byte stores of the epilogue, the column-wise scalar reads of the SIMT
-// reductions and the fragment loads of the MMAs bank-conflict free, and the same bytes stay readable as a plain fp32 tile.
-// A forward result is staged through a dead [128 x 64] tile so that the epilogue gets one sample row per thread
-// (64 / NQ columns each; NQ = 2 or 4 column groups = 256 or 512 threads per CTA); a backward result is consumed
-// element-wise straight from the accumulator fragments.  The weight-gradient GEMM H1^T.D2 contracts over samples and
-// runs on the same mma.sync path with fragments loaded from the same tiles (wgrad_mma_tile below).
+// operand (activations) is split into hi / lo while its fragments are loaded into registers; the B operand (weights) is
+// stored once per task as hi + lo tiles that the tensor cores read from shared memory.  Activation and weight tiles sit
+// in shared memory in a K-major core-matrix layout: 8x4-float core matrices (128 contiguous bytes, rows 16 B apart),
+// next 8 rows at +128 B, next 4 columns at +S_c.  S_c = rows*16 + 16 bytes: the extra 16 B make the row-wise 16-byte
+// stores of the epilogue, the column-wise scalar reads of the SIMT reductions and the fragment loads of the MMAs
+// bank-conflict free, and the same bytes stay readable as a plain fp32 tile.  A forward result is staged through a dead
+// [128 x 64] tile so that the epilogue gets one sample row per thread (64 / NQ columns each; NQ = 2 or 4 column groups =
+// 256 or 512 threads per CTA); a backward result is consumed element-wise straight from the accumulator fragments.  The
+// weight-gradient GEMM H1^T.D2 contracts over samples and runs on warp-level mma.sync with fragments loaded from the
+// same tiles (wgrad_mma_tile below).
 #pragma once
 #include "mlp_tile.cuh"
 
@@ -123,36 +124,85 @@ __device__ __forceinline__ int wgrad_mma_index(int warp, int lane, int nt, int i
 
 // -------------------------------------------------------------------------------------------------------------
 // Layer GEMM  acc += A[128 x 64] . B^T  with B [64(N) x 64(K)] given as hi + lo tiles (K-major, stride SCW), A as one
-// fp32 tile (K-major, stride SCA) split into hi / lo at fragment load.  Warp w owns the m16 tile 16 (w & 7) and the
-// n8 tiles [LNT (w >> 3), +LNT) (LNT = 8 with 8 warps, 4 with 16).  All fragment loads are conflict-free
-// (bank = 4 g + t).  Terms per k-step: lo.hi, hi.lo, then hi.hi.
+// fp32 tile (K-major, stride SCA) split into hi / lo at fragment load, on Hopper's asynchronous warpgroup MMA
+// (wgmma.mma_async m64nNk8 tf32, 3xTF32 split).  Warpgroup q = w >> 2 owns rows [64 (q & 1), +64) and columns
+// [8 LNT (q >> 1), +8 LNT) (LNT = 8 with 8 warps: m64n64; 4 with 16 warps: m64n32), so warp w still owns rows
+// [16 (w & 7), +16) and the n8 tiles [LNT (w >> 3), +LNT), and its accumulator registers have the m16n8 fragment layout
+// (frag_off).  A comes from registers (conflict-free fragment loads, bank = 4 g + t); B is read by the tensor cores from
+// shared memory through a no-swizzle K-major descriptor: core matrices of 8 rows x 16 B, the K-adjacent one at
+// +SCW (leading byte offset), the next 8 rows at +128 B (stride byte offset).  Terms per k-step: lo.hi, hi.lo, then
+// hi.hi.  The hi weight tiles hold tf32-truncated values (the tensor cores ignore the low 13 bits of a tf32 operand
+// either way).
+//
+// layer_gemm_issue issues the MMAs as one commit group per k-step in a rolled loop and waits for each group before the
+// next k-step's fragment loads overwrite the A registers it reads, so only one k-step of A fragments is live.  Keeping
+// more k-steps in flight (to overlap the weight-gradient GEMM) needs distinct registers per k-step, which spilled in the
+// 512-thread kernels and in the dataflow kernel.  The caller still waits (wg_wait) before it reads acc.  The weight tiles must have
+// been made visible to the async proxy (wg_fence_weights, then a barrier) after their generic stores.
+__device__ __forceinline__ uint64_t wg_desc(const unsigned char* p) {
+    const uint32_t a = static_cast<uint32_t>(__cvta_generic_to_shared(p));
+    return (uint64_t)((a & 0x3ffff) >> 4) | ((uint64_t)(SCW >> 4) << 16) | ((uint64_t)(128 >> 4) << 32);   // layout 0: no swizzle
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+constexpr int WG_DEPTH = 0;      // k-step groups left in flight: 0, as the rolled loop reuses the A registers
+__device__ __forceinline__ void wg_wait_depth() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(WG_DEPTH) : "memory"); }
+__device__ __forceinline__ void wg_fence_weights() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+// pins the accumulator registers at this point of the program (no use of them is moved across an issue or a wait)
 template <int LNT>
-__device__ __forceinline__ void layer_gemm(float (&acc)[LNT][4], const unsigned char* __restrict__ a,
-                                           const unsigned char* __restrict__ b_hi, const unsigned char* __restrict__ b_lo,
-                                           int warp, int lane) {
+__device__ __forceinline__ void wg_pin(float (&acc)[LNT][4]) {
+#pragma unroll
+    for (int nt = 0; nt < LNT; ++nt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) asm volatile("" : "+f"(acc[nt][i])::"memory");
+}
+
+template <int LNT>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[LNT][4], const uint32_t (&a)[4], uint64_t desc);
+template <>
+__device__ __forceinline__ void wgmma_tf32<4>(float (&d)[4][4], const uint32_t (&a)[4], uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, 1, 1, 1;\n"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]),
+          "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<8>(float (&d)[8][4], const uint32_t (&a)[4], uint64_t desc) {
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, 1, 1, 1;\n"
+        : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]), "+f"(d[1][3]),
+          "+f"(d[2][0]), "+f"(d[2][1]), "+f"(d[2][2]), "+f"(d[2][3]), "+f"(d[3][0]), "+f"(d[3][1]), "+f"(d[3][2]), "+f"(d[3][3]),
+          "+f"(d[4][0]), "+f"(d[4][1]), "+f"(d[4][2]), "+f"(d[4][3]), "+f"(d[5][0]), "+f"(d[5][1]), "+f"(d[5][2]), "+f"(d[5][3]),
+          "+f"(d[6][0]), "+f"(d[6][1]), "+f"(d[6][2]), "+f"(d[6][3]), "+f"(d[7][0]), "+f"(d[7][1]), "+f"(d[7][2]), "+f"(d[7][3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <int LNT>
+__device__ __forceinline__ void layer_gemm_issue(float (&acc)[LNT][4], const unsigned char* __restrict__ a,
+                                                 const unsigned char* __restrict__ b_hi, const unsigned char* __restrict__ b_lo,
+                                                 int warp, int lane) {
     const int g = lane >> 2, t = lane & 3;
     const unsigned char* ap = a + (warp & 7) * 256 + g * 16 + t * 4;
-    const int bo = (warp >> 3) * LNT * 128 + g * 16 + t * 4;
-#pragma unroll 2
+    const int bo = (warp >> 3) * LNT * 128;
+#pragma unroll 1      // a rolled loop keeps the fragment loads of later k-steps from being hoisted (register pressure)
     for (int s = 0; s < TC_HID / 8; ++s) {
+        const uint64_t dh = wg_desc(b_hi + bo + 2 * s * SCW), dl = wg_desc(b_lo + bo + 2 * s * SCW);      // k-step s
         uint32_t ah[4], al[4];
         const unsigned char* as = ap + 2 * s * SCA;
         split_tf32(*reinterpret_cast<const float*>(as), ah[0], al[0]);
         split_tf32(*reinterpret_cast<const float*>(as + 128), ah[1], al[1]);
         split_tf32(*reinterpret_cast<const float*>(as + SCA), ah[2], al[2]);
         split_tf32(*reinterpret_cast<const float*>(as + SCA + 128), ah[3], al[3]);
-#pragma unroll
-        for (int nt = 0; nt < LNT; ++nt) {
-            const int o = 2 * s * SCW + bo + nt * 128;
-            uint32_t bh[2], bl[2];
-            bh[0] = *reinterpret_cast<const uint32_t*>(b_hi + o) & 0xffffe000u;
-            bh[1] = *reinterpret_cast<const uint32_t*>(b_hi + o + SCW) & 0xffffe000u;
-            bl[0] = *reinterpret_cast<const uint32_t*>(b_lo + o);
-            bl[1] = *reinterpret_cast<const uint32_t*>(b_lo + o + SCW);
-            mma_tf32_16n8k8(acc[nt], al, bh);
-            mma_tf32_16n8k8(acc[nt], ah, bl);
-            mma_tf32_16n8k8(acc[nt], ah, bh);
-        }
+        wg_fence();                                              // the A fragments were just written
+        wgmma_tf32<LNT>(acc, al, dh);
+        wgmma_tf32<LNT>(acc, ah, dl);
+        wgmma_tf32<LNT>(acc, ah, dh);
+        wg_commit();
+        wg_wait_depth();
     }
 }
 template <int LNT>
@@ -160,7 +210,7 @@ __device__ __forceinline__ void zero_frag(float (&acc)[LNT][4]) {
 #pragma unroll
     for (int nt = 0; nt < LNT; ++nt) acc[nt][0] = acc[nt][1] = acc[nt][2] = acc[nt][3] = 0.f;
 }
-// byte offset (in a [128 x 64] activation tile) of the accumulator pair acc[nt][2h], acc[nt][2h + 1] of layer_gemm
+// byte offset (in a [128 x 64] activation tile) of the accumulator pair acc[nt][2h], acc[nt][2h + 1] of layer_gemm_issue
 template <int LNT>
 __device__ __forceinline__ int frag_off(int warp, int lane, int nt, int h) {
     return core_off(16 * (warp & 7) + (lane >> 2) + 8 * h, 8 * (LNT * (warp >> 3) + nt) + 2 * (lane & 3), SCA);
@@ -259,9 +309,7 @@ struct ItemSched {
                     const long long t = clock64();
                     if (t0 == 0) t0 = t;
                     else if (t - t0 > 8000000000ll) {              // ~4 s
-#ifndef PROMP_CHAIN_NO_PRINTF
-                        printf("promp_b200: policy chain item %d waited > 4 s for task %d of the previous stage\n", item, m);
-#endif
+                        // no printf here: a call anywhere in the kernel makes ptxas serialize every wgmma of it
                         __trap();
                     }
                 }
@@ -405,7 +453,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                 w = Sched::ldp4(reinterpret_cast<const float4*>(th + L::W1 + k * HID + 4 * jg));
                 wl = make_float4(w.x - tf32_trunc(w.x), w.y - tf32_trunc(w.y), w.z - tf32_trunc(w.z), w.w - tf32_trunc(w.w));
                 const int off = jg * SCW + (k >> 3) * 128 + (k & 7) * 16;
-                *reinterpret_cast<float4*>(S.W1_hi + off) = w;
+                *reinterpret_cast<float4*>(S.W1_hi + off) = make_float4(tf32_trunc(w.x), tf32_trunc(w.y), tf32_trunc(w.z), tf32_trunc(w.w));
                 *reinterpret_cast<float4*>(S.W1_lo + off) = wl;
             }
             {       // forward operand: tile row = j, K = k; W1[4 kg .. 4 kg + 3][j], lanes run over j
@@ -414,10 +462,11 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                 w = make_float4(Sched::ldp(src), Sched::ldp(src + HID), Sched::ldp(src + 2 * HID), Sched::ldp(src + 3 * HID));
                 wl = make_float4(w.x - tf32_trunc(w.x), w.y - tf32_trunc(w.y), w.z - tf32_trunc(w.z), w.w - tf32_trunc(w.w));
                 const int off = kg * SCW + (j >> 3) * 128 + (j & 7) * 16;
-                *reinterpret_cast<float4*>(S.W1T_hi + off) = w;
+                *reinterpret_cast<float4*>(S.W1T_hi + off) = make_float4(tf32_trunc(w.x), tf32_trunc(w.y), tf32_trunc(w.z), tf32_trunc(w.w));
                 *reinterpret_cast<float4*>(S.W1T_lo + off) = wl;
             }
         }
+        if (reload) wg_fence_weights();      // the weight tiles are read by the wgmma (async) proxy after the barrier
         __syncthreads();          // Ps is in place; every reader of the previous task's hin / hold is done
         if (tid == 0) {
 #pragma unroll
@@ -629,7 +678,9 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         {
             float acc[LNT][4];
             zero_frag<LNT>(acc);
-            layer_gemm<LNT>(acc, S.A0, S.W1T_hi, S.W1T_lo, warp, lane);
+            layer_gemm_issue<LNT>(acc, S.A0, S.W1T_hi, S.W1T_lo, warp, lane);
+            wg_wait();
+            wg_pin<LNT>(acc);
             store_frag<LNT>(acc, S.LO, warp, lane);
         }
         __syncthreads();
@@ -754,7 +805,9 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         {
             float acc[LNT][4];
             zero_frag<LNT>(acc);
-            layer_gemm<LNT>(acc, S.A1, S.W1_hi, S.W1_lo, warp, lane);
+            layer_gemm_issue<LNT>(acc, S.A1, S.W1_hi, S.W1_lo, warp, lane);
+            wg_wait();
+            wg_pin<LNT>(acc);
             __syncthreads();       // every read of H1 (weight gradient) is done before A0 is overwritten
             PCLK(8);
 #pragma unroll
@@ -811,7 +864,7 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs 
 // Tensor-core variant of policy_hvp_kernel (HID = 64).  All six layer GEMMs of the exact Hessian-vector product
 //   forward :  Z2 = H1 W1            RZ2 = R1 W1 + H1 V1
 //   backward:  dH1 = D2 W1^T         CdH1 = C2 W1^T + D2 (ac V1)^T
-// run as layer_gemm (mma.sync 3xTF32, A split into hi / lo at fragment load).  Shared memory cannot hold four
+// run as layer_gemm_issue (wgmma 3xTF32, A split into hi / lo at fragment load).  Shared memory cannot hold four
 // activation tiles next to hi+lo copies of four weight tiles, so the B (weight) buffer is time-multiplexed:
 // [W1^T, V1^T] for the forward MMAs, re-filled with [W1, ac V1] for the backward MMAs (66 KB from L2 twice per 128-row
 // tile).  The forward results Z2 / RZ2 are staged in T2a / T2b (the thread that reads an element back writes H2 / R2
@@ -931,7 +984,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
 #pragma unroll
         for (int d = 0; d < DA; ++d) rls[d] = S.Vs[SL::LS + d] * hin.ls_mask[d];
     };
-    // (re)fill the weight buffer from L2: forward = [W1^T, V1^T], backward = [W1, ac*V1], each as hi (fp32) + lo
+    // (re)fill the weight buffer from L2: forward = [W1^T, V1^T], backward = [W1, ac*V1], each as hi (tf32-truncated) + lo
     // 4 elements per thread and buffer: one conflict-free 16-byte shared-memory store each (the element-wise version paid a
     // 4-way bank conflict on every forward-layout store: 1.0 M of the kernel's 1.2 M conflicts in the round-1 profile)
     auto load_weights = [&](bool fwd) {
@@ -952,13 +1005,14 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                 v = make_float4(ac * v.x, ac * v.y, ac * v.z, ac * v.w);
                 off = jg * SCW + (k >> 3) * 128 + (k & 7) * 16;
             }
-            *reinterpret_cast<float4*>(S.WB[0] + off) = w;
+            *reinterpret_cast<float4*>(S.WB[0] + off) = make_float4(tf32_trunc(w.x), tf32_trunc(w.y), tf32_trunc(w.z), tf32_trunc(w.w));
             *reinterpret_cast<float4*>(S.WB[1] + off) =
                 make_float4(w.x - tf32_trunc(w.x), w.y - tf32_trunc(w.y), w.z - tf32_trunc(w.z), w.w - tf32_trunc(w.w));
-            *reinterpret_cast<float4*>(S.WB[2] + off) = v;
+            *reinterpret_cast<float4*>(S.WB[2] + off) = make_float4(tf32_trunc(v.x), tf32_trunc(v.y), tf32_trunc(v.z), tf32_trunc(v.w));
             *reinterpret_cast<float4*>(S.WB[3] + off) =
                 make_float4(v.x - tf32_trunc(v.x), v.y - tf32_trunc(v.y), v.z - tf32_trunc(v.z), v.w - tf32_trunc(v.w));
         }
+        wg_fence_weights();      // read by the wgmma (async) proxy after the caller's next barrier
     };
     auto flush = [&](int m) {
         sc.clk(3);
@@ -1138,14 +1192,18 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
         {
             float acc[LNT][4];
             zero_frag<LNT>(acc);
-            layer_gemm<LNT>(acc, S.H1, S.WB[0], S.WB[1], warp, lane);
+            layer_gemm_issue<LNT>(acc, S.H1, S.WB[0], S.WB[1], warp, lane);
+            wg_wait();
+            wg_pin<LNT>(acc);
             store_frag<LNT>(acc, S.T2a, warp, lane);
             zero_frag<LNT>(acc);
-            layer_gemm<LNT>(acc, S.R1, S.WB[0], S.WB[1], warp, lane);
-            layer_gemm<LNT>(acc, S.H1, S.WB[2], S.WB[3], warp, lane);
+            layer_gemm_issue<LNT>(acc, S.R1, S.WB[0], S.WB[1], warp, lane);
+            layer_gemm_issue<LNT>(acc, S.H1, S.WB[2], S.WB[3], warp, lane);
+            wg_wait();
+            wg_pin<LNT>(acc);
             store_frag<LNT>(acc, S.T2b, warp, lane);
         }
-        __syncthreads();       // also: every read of WB is done before MUP (aliasing WB[0..1]) is written
+        __syncthreads();       // also: every MMA read of WB has completed before MUP (aliasing WB[0..1]) is written
         float h2[CW], r2[CW];
         load_row<CW>(S.T2a, r, c0, h2);
         load_row<CW>(S.T2b, r, c0, r2);
@@ -1302,9 +1360,12 @@ float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
             float dacc[LNT][4], cacc[LNT][4];
             zero_frag<LNT>(dacc);
             zero_frag<LNT>(cacc);
-            layer_gemm<LNT>(dacc, S.T2a, S.WB[0], S.WB[1], warp, lane);
-            layer_gemm<LNT>(cacc, S.T2b, S.WB[0], S.WB[1], warp, lane);
-            layer_gemm<LNT>(cacc, S.T2a, S.WB[2], S.WB[3], warp, lane);
+            layer_gemm_issue<LNT>(dacc, S.T2a, S.WB[0], S.WB[1], warp, lane);
+            layer_gemm_issue<LNT>(cacc, S.T2b, S.WB[0], S.WB[1], warp, lane);
+            layer_gemm_issue<LNT>(cacc, S.T2a, S.WB[2], S.WB[3], warp, lane);
+            wg_wait();
+            wg_pin<LNT>(dacc);
+            wg_pin<LNT>(cacc);
             __syncthreads();       // all reads of H1 / R1 / T2a are done before H1 and X (aliasing T2a) are overwritten
 #pragma unroll
             for (int nt = 0; nt < LNT; ++nt)
