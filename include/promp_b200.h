@@ -44,7 +44,10 @@ enum {
     PROMP_ENV_POINT = 1,
     PROMP_ENV_CHEETAH_DIR = 2,
     PROMP_ENV_POINT_WALLS = 3,     /* envs/point_envs/point_env_2d_walls.py: two circular walls with one gap each      */
-    PROMP_ENV_POINT_MOMENTUM = 4   /* envs/point_envs/point_env_2d_momentum.py: actions accelerate, obs = (pos, vel)   */
+    PROMP_ENV_POINT_MOMENTUM = 4,  /* envs/point_envs/point_env_2d_momentum.py: actions accelerate, obs = (pos, vel)   */
+    PROMP_ENV_WALKER = 5,          /* envs/mujoco_envs/walker2d_rand_vel.py / walker2d_rand_direc.py [analytic surrogate,
+                                      obs 17 / act 6, early done when the torso falls]                                  */
+    PROMP_ENV_SWIMMER = 6          /* envs/mujoco_envs/swimmer_rand_vel.py [analytic surrogate, obs 8 / act 2]           */
 };
 /* MetaPointEnvCorner.reward_type (point_env_2d_corner.py:13-16) */
 enum { PROMP_REWARD_SPARSE = 0, PROMP_REWARD_DENSE = 1, PROMP_REWARD_DENSE_SQUARED = 2 };
@@ -63,10 +66,13 @@ int promp_version(void);
 
 /* Number of policy parameters P for (obs_dim, act_dim, hidden,hidden). */
 int promp_num_params(int obs_dim, int act_dim, int hidden);
-/* State floats per env for init_state / final_state: 2 (point envs; 4 = pos, vel for the momentum env), 18 (cheetah: qpos[9] qvel[9]). */
+/* State floats per env for init_state / final_state: 2 (point envs; 4 = pos, vel for the momentum env), 18 (cheetah, walker:
+ * qpos[9] qvel[9]), 10 (swimmer: qpos[5] qvel[5]). */
 int promp_env_state_dim(int env_kind);
 /* Floats per task in task_params: 2 (point corner / momentum goal), 0 -> pass 1 dummy (point), 1 (cheetah: direction or goal
- * velocity), 6 (walls: goal, gap_1, gap_2). */
+ * velocity), 6 (walls: goal, gap_1, gap_2), 2 (walker: direction or goal velocity, then the reward mode 0 = Walker2DRandDirec
+ * [dir * forward_vel + 1], 1 = Walker2DRandVel [-|forward_vel - goal| + 15]; reward_type is not read), 1 (swimmer: goal
+ * velocity). */
 int promp_env_task_dim(int env_kind);
 
 /*
@@ -94,6 +100,9 @@ int promp_env_task_dim(int env_kind);
  *        [3,M,E,H]  for the cheetah with reward_type 1 = HalfCheetahRandVel (mujoco_envs/half_cheetah_rand_vel.py:30-40:
  *                   reward_run = -|forward_vel - task|, task = goal velocity): third channel = forward_vel;
  *                   reward_type 0 = HalfCheetahRandDirec (reward_run = task * forward_vel, task = direction)
+ *        [2,M,E,H]  swimmer (mujoco_envs/swimmer_rand_vel.py:30-39, reward_type 0): reward_fwd, reward_ctrl
+ *   The walker records fixed-horizon trajectories here (done only at t = H-1, its fall rule is not applied); its
+ *   early-terminating sampler is promp_rollout_early_term.
  *   log_std_out [M,Da]  the per-task reported log_std (constant over the phase)
  *   final_state [M,E,state_dim] or NULL
  */
@@ -134,7 +143,9 @@ int promp_env_observe(int env_kind, int n_env, const float* state, float* obs, v
  * promp_rollout_early_term: like promp_rollout, but every env slot records a TIMELINE of `timeline_len` steps
  *   (obs/act/mean [M,E,T,.], rew [M,E,T], done [M,E,T] u8); a path ends when the env reports done or after `horizon` steps;
  *   the slot is reset at once (U(-2,2)^2 from Philox keyed by (env, step) - the host numpy stream cannot be followed when the
- *   number of resets is data-dependent) and the next recorded observation is the reset state.  timeline_len >= 2*horizon - 1
+ *   number of resets is data-dependent) and the next recorded observation is the reset state.  env_kind PROMP_ENV_POINT or
+ *   PROMP_ENV_WALKER (walker2d_rand_*.py: done when the torso falls; reset = init_qpos + U(-.005,.005)^9, U(-.005,.005)^9
+ *   from Philox keyed by (env, step, coordinate); task_params [M, 2] select the reward mode).  timeline_len >= 2*horizon - 1
  *   guarantees that promp_paths_finalize finds enough completed samples.
  * promp_paths_finalize: applies the reference's rule to the timelines: t* = first step at which the paths completed so far
  *   hold >= target_samples (= M*E*H) samples; task m keeps the paths completing at steps <= t*, in (step, env index) order

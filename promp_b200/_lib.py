@@ -13,6 +13,9 @@ LIB_PATH = os.environ.get('PROMP_B200_LIB', os.path.join(_HERE, 'libpromp_b200.s
 
 # enums (mirror include/promp_b200.h)
 ENV_POINT_CORNER, ENV_POINT, ENV_CHEETAH_DIR, ENV_POINT_WALLS, ENV_POINT_MOMENTUM = 0, 1, 2, 3, 4
+ENV_WALKER, ENV_SWIMMER = 5, 6
+EARLY_TERM_ENVS = (ENV_POINT, ENV_WALKER)        # env kinds whose paths end on `done` (variable-length paths)
+INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write env_infos channels
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE = 0, 1, 2, 3
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE = 0, 1

@@ -4,6 +4,10 @@
 //   cheetah      : MuJoCo-free HalfCheetahRandDirec surrogate; reward / obs / reset / task spec follow
 //                  ref envs/mujoco_envs/half_cheetah_rand_direc.py:14-53, the dynamics are defined in
 //                  DESIGN.md (restated on the CPU in oracle/cheetah_surrogate.py).
+//   walker       : MuJoCo-free Walker2DRandVel / Walker2DRandDirec surrogate (ref envs/mujoco_envs/walker2d_rand_vel.py,
+//                  walker2d_rand_direc.py), early `done` when the torso falls.
+//   swimmer      : MuJoCo-free SwimmerRandVel surrogate (ref envs/mujoco_envs/swimmer_rand_vel.py).
+//                  Both restated on the CPU in oracle/locomotion_surrogates.py.
 //   NormalizedEnv: ref envs/normalized_env.py:109-117 (action affine map + clip; obs / reward
 //                  normalisation are off by default, :23-24, and out of scope).
 #pragma once
@@ -26,6 +30,12 @@ template <> struct EnvTraits<PROMP_ENV_POINT_WALLS> {
 };
 template <> struct EnvTraits<PROMP_ENV_POINT_MOMENTUM> {
     static constexpr int DO = 4, DA = 2, SD = 4, TD = 2, NINFO = 0;       // state = obs = (pos, vel)
+};
+template <> struct EnvTraits<PROMP_ENV_WALKER> {
+    static constexpr int DO = 17, DA = 6, SD = 18, TD = 2, NINFO = 0;     // task = (direction | goal velocity, mode)
+};
+template <> struct EnvTraits<PROMP_ENV_SWIMMER> {
+    static constexpr int DO = 8, DA = 2, SD = 10, TD = 1, NINFO = 2;      // info = reward_fwd, reward_ctrl
 };
 
 // NormalizedEnv.step action map, same evaluation order as the reference expression
@@ -268,5 +278,163 @@ __device__ __forceinline__ void step_warp(const JointConst& jc, float u, float& 
     reward = r_ctrl + r_run;
 }
 }  // namespace cheetah
+
+// ------------------------------------------------------------------ walker2d surrogate
+// MuJoCo-free Walker2DRandVel / Walker2DRandDirec: obs / reward / done / reset follow ref envs/mujoco_envs/
+// walker2d_rand_vel.py:32-55 and walker2d_rand_direc.py:32-55; the dynamics are defined in DESIGN.md §3.4 and restated
+// on the CPU in oracle/locomotion_surrogates.py.  State = qpos[9] ++ qvel[9] with root (x, z, pitch) like the cheetah;
+// the torso is an inverted pendulum, so a path ends (done) once it has fallen.
+namespace walker {
+constexpr int NJ = 6;
+constexpr float HS = 0.002f, DT = 0.016f;
+constexpr int FRAME_SKIP = 8;
+static __device__ __constant__ const float G[8] = {6.0f, 5.0f, 3.0f, 6.0f, 5.0f, 3.0f, 0.f, 0.f};
+static __device__ __constant__ const float K[8] = {20.0f, 16.0f, 10.0f, 20.0f, 16.0f, 10.0f, 0.f, 0.f};
+static __device__ __constant__ const float D[8] = {3.0f, 2.5f, 1.5f, 3.0f, 2.5f, 1.5f, 0.f, 0.f};
+static __device__ __constant__ const float C[8] = {0.8f, 0.6f, 0.3f, 0.8f, 0.6f, 0.3f, 0.f, 0.f};
+static __device__ __constant__ const float PH[8] = {0.4f, -0.3f, 0.9f, -0.4f, 0.3f, -0.9f, 0.f, 0.f};
+static __device__ __constant__ const float P[8] = {1.2f, -0.8f, 0.5f, -1.0f, 0.9f, -0.6f, 0.f, 0.f};
+constexpr float BX = 1.0f, Z0 = 1.25f, KZ = 60.0f, DZ = 12.0f, LZ = 0.5f, AP = 5.0f, DP = 0.5f;
+
+struct JointConst {
+    float g, k, d, c, ph, p;
+};
+__device__ __forceinline__ JointConst joint_const(int j) {
+    int i = j < NJ ? j : 7;
+    return JointConst{G[i], K[i], D[i], C[i], PH[i], P[i]};
+}
+
+// walker2d_rand_*.py:36-37: done = not (0.8 < height < 2.0 and -1 < angle < 1)
+__device__ __forceinline__ bool is_done(float z, float ang) {
+    return !(z > 0.8f && z < 2.0f && ang > -1.0f && ang < 1.0f);
+}
+// obs clips qvel to [-10, 10] (walker2d_rand_*.py:42-45)
+__device__ __forceinline__ float clip_vel(float v) { return fminf(fmaxf(v, -10.0f), 10.0f); }
+
+// mode 0: RandDirec, reward = dir * fwd_vel + 1 - 1e-3 |u|^2;  mode 1: RandVel, reward = -|fwd_vel - goal| + 15 - 1e-3 |u|^2
+__device__ __forceinline__ float reward(float fwd_vel, float su, float task, int mode) {
+    return (mode ? -fabsf(fwd_vel - task) + 15.0f : task * fwd_vel + 1.0f) - 1e-3f * su;
+}
+
+// Serial version (one thread per env): state = qpos[9] ++ qvel[9]; u[6] already clipped.
+__device__ inline void step_serial(float* st, const float* u, float task, int mode, float& rew, float& fwd_vel) {
+    const float x0 = st[0];
+    float twist = 0.f, su = 0.f;
+    for (int j = 0; j < NJ; ++j) twist = twist + P[j] * u[j];
+    for (int s = 0; s < FRAME_SKIP; ++s) {
+        float thrust = 0.f, lift = 0.f;
+        const float pitch = st[2];
+        for (int j = 0; j < NJ; ++j) {
+            float q = st[3 + j], qd = st[12 + j];
+            const float acc = G[j] * u[j] - K[j] * q - D[j] * qd;
+            qd = qd + HS * acc;
+            q = q + HS * qd;
+            st[3 + j] = q;
+            st[12 + j] = qd;
+            float sn, cs;
+            __sincosf(q + pitch + PH[j], &sn, &cs);
+            thrust = thrust + C[j] * qd * sn;
+            lift = lift + C[j] * qd * cs;
+        }
+        float psn, pcs;
+        __sincosf(pitch, &psn, &pcs);
+        const float xd = st[9] + HS * (thrust - BX * st[9]);
+        st[9] = xd;
+        st[0] = st[0] + HS * xd;
+        const float zd = st[10] + HS * (KZ * (Z0 * pcs - st[1]) - DZ * st[10] + LZ * lift);
+        st[10] = zd;
+        st[1] = st[1] + HS * zd;
+        const float pd = st[11] + HS * (AP * psn + twist - DP * st[11]);
+        st[11] = pd;
+        st[2] = pitch + HS * pd;
+    }
+    for (int j = 0; j < NJ; ++j) su += u[j] * u[j];
+    fwd_vel = (st[0] - x0) / DT;
+    rew = reward(fwd_vel, su, task, mode);
+}
+
+// Warp version, the cheetah's decomposition (cheetah::step_warp): lane j < 6 owns joint j, the root floats are
+// replicated.  The pitch depends on the torques only (constant over the sub-steps), so every lane integrates it; x and z
+// are LINEAR in the per-joint thrust / lift, so every lane integrates its own joint's driven response from zero and the
+// homogeneous part (with the replicated Z0*cos(pitch) drive) from the real initial conditions; one 8-lane reduction per
+// env step adds them up.
+__device__ __forceinline__ void step_warp(const JointConst& jc, float u, float& q, float& qd, float (&root)[6], float task, int mode,
+                                          float& rew, float& fwd_vel) {
+    const float x0 = root[0];
+    const float twist = cheetah::sum8(jc.p * u);
+    const float su = cheetah::sum8(u * u);
+    float xdh = root[3], xh = root[0], zdh = root[4], zh = root[1];
+    float xdp = 0.f, xp = 0.f, zdp = 0.f, zp = 0.f;
+    float pitch = root[2], pd = root[5];
+#pragma unroll
+    for (int s = 0; s < FRAME_SKIP; ++s) {
+        const float acc = jc.g * u - jc.k * q - jc.d * qd;
+        qd = qd + HS * acc;
+        q = q + HS * qd;
+        float sn, cs, psn, pcs;
+        __sincosf(q + pitch + jc.ph, &sn, &cs);
+        __sincosf(pitch, &psn, &pcs);
+        const float t = jc.c * qd * sn, l = jc.c * qd * cs;
+        xdp = xdp + HS * (t - BX * xdp);
+        xp = xp + HS * xdp;
+        zdp = zdp + HS * (LZ * l - KZ * zp - DZ * zdp);
+        zp = zp + HS * zdp;
+        xdh = xdh + HS * (0.f - BX * xdh);
+        xh = xh + HS * xdh;
+        zdh = zdh + HS * (KZ * (Z0 * pcs - zh) - DZ * zdh);
+        zh = zh + HS * zdh;
+        pd = pd + HS * (AP * psn + twist - DP * pd);
+        pitch = pitch + HS * pd;
+    }
+    root[3] = xdh + cheetah::sum8(xdp);
+    root[0] = xh + cheetah::sum8(xp);
+    root[4] = zdh + cheetah::sum8(zdp);
+    root[1] = zh + cheetah::sum8(zp);
+    root[5] = pd;
+    root[2] = pitch;
+    fwd_vel = (root[0] - x0) / DT;
+    rew = reward(fwd_vel, su, task, mode);
+}
+}  // namespace walker
+
+// ------------------------------------------------------------------ swimmer surrogate
+// MuJoCo-free SwimmerRandVel: obs / reward / reset follow ref envs/mujoco_envs/swimmer_rand_vel.py:30-50 (reward_fwd =
+// |fwd_vel - goal| with the reference's sign), the dynamics are defined in DESIGN.md §3.4 (CPU: oracle/
+// locomotion_surrogates.py).  State = qpos (x, y, rot, q0, q1) ++ qvel.  Two joints: the whole step is cheap enough to run
+// replicated in every lane of the env's warp (no reductions), and the single-step kernel runs the same function.
+namespace swimmer {
+constexpr float HS = 0.01f, DT = 0.04f;
+constexpr int FRAME_SKIP = 4;
+constexpr float G0 = 10.0f, G1 = 10.0f, K0 = 4.0f, K1 = 4.0f, D0 = 1.0f, D1 = 1.0f, P0 = 0.5f, P1 = -0.5f;
+constexpr float CS = 0.02f, DR = 2.0f, BV = 1.0f;
+
+__device__ __forceinline__ void step(float (&st)[10], float u0, float u1, float goal, float& rew, float& r_fwd, float& r_ctrl) {
+    const float x0 = st[0];
+    const float twist = P0 * u0 + P1 * u1;
+#pragma unroll
+    for (int s = 0; s < FRAME_SKIP; ++s) {
+        float qd0 = st[8] + HS * (G0 * u0 - K0 * st[3] - D0 * st[8]);
+        const float q0 = st[3] + HS * qd0;
+        float qd1 = st[9] + HS * (G1 * u1 - K1 * st[4] - D1 * st[9]);
+        const float q1 = st[4] + HS * qd1;
+        st[3] = q0, st[8] = qd0, st[4] = q1, st[9] = qd1;
+        const float thrust = CS * (q0 * qd1 - q1 * qd0);
+        const float rot = st[2];
+        const float rd = st[7] + HS * (twist - DR * st[7]);
+        float sn, cs;
+        __sincosf(rot, &sn, &cs);
+        const float xd = st[5] + HS * (thrust * cs - BV * st[5]);
+        const float yd = st[6] + HS * (thrust * sn - BV * st[6]);
+        st[5] = xd, st[6] = yd, st[7] = rd;
+        st[0] = st[0] + HS * xd;
+        st[1] = st[1] + HS * yd;
+        st[2] = rot + HS * rd;
+    }
+    const float fwd_vel = (st[0] - x0) / DT;
+    r_fwd = fabsf(fwd_vel - goal);
+    r_ctrl = -1e-4f * (u0 * u0 + u1 * u1);
+    rew = r_fwd + r_ctrl;
+}
+}  // namespace swimmer
 
 }  // namespace promp

@@ -71,6 +71,32 @@ __device__ unsigned long long g_ro_clk[16];
 #define RCLK(i)
 #endif
 
+// walker reset_model (walker2d_rand_*.py:47-52): qpos = init_qpos + U(-.005,.005)^9 (init_qpos z = 1.25, all else 0),
+// qvel = U(-.005,.005)^9.  Lane i < 9 draws coordinate i from Philox counter (env, ctr + i); the result is spread over the
+// warp like the cheetah's reset (root replicated, lane j < 6 keeps joint j).
+__device__ __forceinline__ void walker_reset(const RolloutArgs& A, int64_t env_id, uint32_t ctr, uint32_t tag, int lane, float& q,
+                                             float& qd, float (&root)[6]) {
+    float pos = 0.f, vel = 0.f;
+    if (lane < 9) {
+        uint32_t r[4];
+        Philox::gen((uint32_t)env_id, ctr + (uint32_t)lane, (uint32_t)A.stream_id, tag | (uint32_t)((A.stream_id >> 32) & 0xffffffu),
+                    A.seed, r);
+        pos = -0.005f + 0.01f * u01(r[0]);
+        vel = -0.005f + 0.01f * u01(r[1]);
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        root[i] = __shfl_sync(0xffffffffu, pos, i);
+        root[3 + i] = __shfl_sync(0xffffffffu, vel, i);
+    }
+    root[1] += 1.25f;
+    const int jl = lane & 7;
+    const float qq = __shfl_sync(0xffffffffu, pos, 3 + (jl < 6 ? jl : 0));
+    const float qv = __shfl_sync(0xffffffffu, vel, 3 + (jl < 6 ? jl : 0));
+    q = jl < 6 ? qq : 0.f;
+    qd = jl < 6 ? qv : 0.f;
+}
+
 template <int KIND, int HID>
 __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
     using T = EnvTraits<KIND>;
@@ -125,10 +151,14 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
 
     // env state registers
     float sx = 0.f, sy = 0.f, vx = 0.f, vy = 0.f;   // point envs (vx, vy: momentum env)
-    float q = 0.f, qd = 0.f, root[6] = {0, 0, 0, 0, 0, 0};   // cheetah: lane's joint (lane&7) + replicated root
+    float q = 0.f, qd = 0.f, root[6] = {0, 0, 0, 0, 0, 0};   // cheetah / walker: lane's joint (lane&7) + replicated root
     cheetah::JointConst jc = cheetah::joint_const(lane & 7);
+    walker::JointConst wjc = walker::joint_const(lane & 7);
+    float sw[10];                                            // swimmer: qpos[5] ++ qvel[5], replicated in every lane
+#pragma unroll
+    for (int k = 0; k < 10; ++k) sw[k] = 0.f;
 
-    if (KIND == PROMP_ENV_CHEETAH_DIR) {
+    if (KIND == PROMP_ENV_CHEETAH_DIR || KIND == PROMP_ENV_WALKER) {
         const int jl = lane & 7;
         if (A.init_state) {
             const float* s0 = A.init_state + env_id * SD;
@@ -136,6 +166,8 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             root[3] = s0[9]; root[4] = s0[10]; root[5] = s0[11];
             q = jl < 6 ? s0[3 + jl] : 0.f;
             qd = jl < 6 ? s0[12 + jl] : 0.f;
+        } else if (KIND == PROMP_ENV_WALKER) {
+            walker_reset(A, env_id, 0u, 0x52000000u, lane, q, qd, root);
         } else {
             // reset_model (half_cheetah_rand_direc.py:49-53): qpos = U(-.1,.1)^9, qvel = .1*N(0,1)^9
             float pos = 0.f, vel = 0.f;
@@ -157,6 +189,22 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             float qv = __shfl_sync(0xffffffffu, vel, 3 + (jl < 6 ? jl : 0));
             q = jl < 6 ? qq : 0.f;
             qd = jl < 6 ? qv : 0.f;
+        }
+    } else if (KIND == PROMP_ENV_SWIMMER) {
+        if (A.init_state) {
+#pragma unroll
+            for (int k = 0; k < 10; ++k) sw[k] = A.init_state[env_id * SD + k];
+        } else {
+            // reset_model (swimmer_rand_vel.py:41-46): qpos = U(-.1,.1)^5, qvel = U(-.1,.1)^5 (every lane draws the same)
+#pragma unroll
+            for (int blk = 0; blk < 3; ++blk) {
+                uint32_t r[4];
+                Philox::gen((uint32_t)env_id, (uint32_t)blk, (uint32_t)A.stream_id,
+                            0x52000000u | (uint32_t)((A.stream_id >> 32) & 0xffffffu), A.seed, r);
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    if (blk * 4 + i < 10) sw[blk * 4 + i] = -0.1f + 0.2f * u01(r[i]);
+            }
         }
     } else {
         if (A.init_state) {
@@ -184,6 +232,25 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             if (lane < 6) {
                 S.obs[2 + lane] = q;
                 S.obs[11 + lane] = qd;
+            }
+        } else if (KIND == PROMP_ENV_WALKER) {
+            // obs = qpos[1:] ++ clip(qvel, -10, 10) (walker2d_rand_*.py:42-45)
+            if (lane == 0) {
+                S.obs[0] = root[1]; S.obs[1] = root[2];
+                S.obs[8] = walker::clip_vel(root[3]); S.obs[9] = walker::clip_vel(root[4]); S.obs[10] = walker::clip_vel(root[5]);
+            }
+            if (lane < 6) {
+                S.obs[2 + lane] = q;
+                S.obs[11 + lane] = walker::clip_vel(qd);
+            }
+        } else if (KIND == PROMP_ENV_SWIMMER) {
+            // obs = qpos[2:] ++ qvel (swimmer_rand_vel.py:37-40)
+            if (lane < 8) {
+                float v = 0.f;
+#pragma unroll
+                for (int k = 0; k < 8; ++k)
+                    if (lane == k) v = sw[2 + k];
+                S.obs[lane] = v;
             }
         } else if (lane == 0) {
             S.obs[0] = sx;
@@ -239,7 +306,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             __syncwarp();
             RCLK(2);
             // ---- layer 1: h2 = tanh(h1 W1 + b1); NACC accumulators per output for ILP (4 where the registers allow it)
-            constexpr int NACC = (KIND == PROMP_ENV_CHEETAH_DIR) ? 2 : 4;
+            constexpr int NACC = (KIND == PROMP_ENV_CHEETAH_DIR || KIND == PROMP_ENV_WALKER) ? 2 : 4;
             float acc[NU][NACC];
 #pragma unroll
             for (int u = 0; u < NU; ++u) {
@@ -314,6 +381,34 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
                 r = point_walls_step(sx, sy, a[0], a[1], task, A.reward_type, A.normalized != 0);
             } else if (KIND == PROMP_ENV_POINT_MOMENTUM) {
                 r = point_momentum_step(sx, sy, vx, vy, a[0], a[1], task[0], task[1], pcfg);
+            } else if (KIND == PROMP_ENV_WALKER) {
+                float al = 0.f;
+                const int jl = lane & 7;
+#pragma unroll
+                for (int d = 0; d < DA; ++d)
+                    if (jl == d) al = a[d];
+                const float u_l = jl < 6 ? (A.normalized ? normalized_action(al, -1.f, 1.f) : fminf(fmaxf(al, -1.f), 1.f)) : 0.f;
+                float fwd_vel;
+                walker::step_warp(wjc, u_l, q, qd, root, task[0], task[TD - 1] != 0.f, r, fwd_vel);
+                if (A.early_term) {
+                    // as MetaPointEnv above: the root is replicated, so the done decision is warp-uniform
+                    ++path_ts;
+                    const bool fin = walker::is_done(root[1], root[2]) || path_ts >= A.horizon;
+                    if (lane == 0) S.st_done[tt] = fin ? 1 : 0;
+                    if (fin) {
+                        walker_reset(A, env_id, (uint32_t)(t0 + tt) << 4, 0x53000000u, lane, q, qd, root);
+                        path_ts = 0;
+                    }
+                }
+            } else if (KIND == PROMP_ENV_SWIMMER) {
+                const float u0 = A.normalized ? normalized_action(a[0], -1.f, 1.f) : fminf(fmaxf(a[0], -1.f), 1.f);
+                const float u1 = A.normalized ? normalized_action(a[1], -1.f, 1.f) : fminf(fmaxf(a[1], -1.f), 1.f);
+                float r_fwd, r_ctrl;
+                swimmer::step(sw, u0, u1, task[0], r, r_fwd, r_ctrl);
+                if (lane == 0) {
+                    S.st_info[tt] = r_fwd;
+                    S.st_info[T_CH + tt] = r_ctrl;
+                }
             } else {
                 float al = 0.f;
                 const int jl = lane & 7;
@@ -369,7 +464,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
 #endif
     if (A.final_state) {
         float* fs = A.final_state + env_id * SD;
-        if (KIND == PROMP_ENV_CHEETAH_DIR) {
+        if (KIND == PROMP_ENV_CHEETAH_DIR || KIND == PROMP_ENV_WALKER) {
             if (lane == 0) {
                 fs[0] = root[0]; fs[1] = root[1]; fs[2] = root[2];
                 fs[9] = root[3]; fs[10] = root[4]; fs[11] = root[5];
@@ -378,6 +473,10 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
                 fs[3 + lane] = q;
                 fs[12 + lane] = qd;
             }
+        } else if (KIND == PROMP_ENV_SWIMMER) {
+            if (lane == 0)
+#pragma unroll
+                for (int k = 0; k < 10; ++k) fs[k] = sw[k];
         } else if (lane == 0) {
             fs[0] = sx;
             fs[1] = sy;
@@ -413,6 +512,25 @@ __global__ void env_step_kernel(int reward_type, float radius, int normalized, i
         PointCornerCfg cfg{reward_type, radius, normalized != 0};
         r = point_momentum_step(st[0], st[1], st[SD > 2 ? 2 : 0], st[SD > 3 ? 3 : 1], a[0], a[1], task_params[(int64_t)i * TD],
                                 task_params[(int64_t)i * TD + 1], cfg);
+    } else if (KIND == PROMP_ENV_WALKER) {
+        float u[DA], fv;
+#pragma unroll
+        for (int k = 0; k < DA; ++k) u[k] = normalized ? normalized_action(a[k], -1.f, 1.f) : fminf(fmaxf(a[k], -1.f), 1.f);
+        walker::step_serial(st, u, task_params[(int64_t)i * TD], task_params[(int64_t)i * TD + TD - 1] != 0.f, r, fv);
+        dn = walker::is_done(st[1], st[2]);
+    } else if (KIND == PROMP_ENV_SWIMMER) {
+        float s10[10], rf, rc;
+#pragma unroll
+        for (int k = 0; k < 10; ++k) s10[k] = st[k < SD ? k : 0];
+        const float u0 = normalized ? normalized_action(a[0], -1.f, 1.f) : fminf(fmaxf(a[0], -1.f), 1.f);
+        const float u1 = normalized ? normalized_action(a[DA > 1 ? 1 : 0], -1.f, 1.f) : fminf(fmaxf(a[DA > 1 ? 1 : 0], -1.f), 1.f);
+        swimmer::step(s10, u0, u1, task_params[(int64_t)i * TD], r, rf, rc);
+#pragma unroll
+        for (int k = 0; k < SD; ++k) st[k] = s10[k < 10 ? k : 0];
+        if (info) {
+            info[i] = rf;
+            info[n_env + i] = rc;
+        }
     } else {
         float u[DA], rr, rc, fv;
 #pragma unroll
@@ -441,6 +559,14 @@ __global__ void env_step_kernel(int reward_type, float radius, int normalized, i
         for (int k = 0; k < 8; ++k) next_obs[(int64_t)i * DO + k] = st[1 + k];
 #pragma unroll
         for (int k = 0; k < 9; ++k) next_obs[(int64_t)i * DO + 8 + k] = st[9 + k];
+    } else if (KIND == PROMP_ENV_WALKER) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) next_obs[(int64_t)i * DO + k] = st[1 + k];
+#pragma unroll
+        for (int k = 0; k < 9; ++k) next_obs[(int64_t)i * DO + 8 + k] = walker::clip_vel(st[9 + k]);
+    } else if (KIND == PROMP_ENV_SWIMMER) {
+#pragma unroll
+        for (int k = 0; k < DO; ++k) next_obs[(int64_t)i * DO + k] = st[2 + k];
     } else {
 #pragma unroll
         for (int k = 0; k < DO; ++k) next_obs[(int64_t)i * DO + k] = st[k];       // point envs: obs = state
@@ -455,6 +581,11 @@ __global__ void env_observe_kernel(int n_env, const float* state, float* obs) {
     if (KIND == PROMP_ENV_CHEETAH_DIR) {
         for (int k = 0; k < 8; ++k) obs[(int64_t)i * T::DO + k] = state[(int64_t)i * T::SD + 1 + k];
         for (int k = 0; k < 9; ++k) obs[(int64_t)i * T::DO + 8 + k] = state[(int64_t)i * T::SD + 9 + k];
+    } else if (KIND == PROMP_ENV_WALKER) {
+        for (int k = 0; k < 8; ++k) obs[(int64_t)i * T::DO + k] = state[(int64_t)i * T::SD + 1 + k];
+        for (int k = 0; k < 9; ++k) obs[(int64_t)i * T::DO + 8 + k] = walker::clip_vel(state[(int64_t)i * T::SD + 9 + k]);
+    } else if (KIND == PROMP_ENV_SWIMMER) {
+        for (int k = 0; k < T::DO; ++k) obs[(int64_t)i * T::DO + k] = state[(int64_t)i * T::SD + 2 + k];
     } else {
         for (int k = 0; k < T::DO; ++k) obs[(int64_t)i * T::DO + k] = state[(int64_t)i * T::SD + k];
     }
@@ -479,6 +610,8 @@ extern "C" int promp_env_state_dim(int env_kind) {
         case PROMP_ENV_CHEETAH_DIR: return 18;
         case PROMP_ENV_POINT_WALLS: return 2;
         case PROMP_ENV_POINT_MOMENTUM: return 4;
+        case PROMP_ENV_WALKER: return 18;
+        case PROMP_ENV_SWIMMER: return 10;
     }
     return -1;
 }
@@ -489,6 +622,8 @@ extern "C" int promp_env_task_dim(int env_kind) {
         case PROMP_ENV_CHEETAH_DIR: return 1;
         case PROMP_ENV_POINT_WALLS: return 6;
         case PROMP_ENV_POINT_MOMENTUM: return 2;
+        case PROMP_ENV_WALKER: return 2;
+        case PROMP_ENV_SWIMMER: return 1;
     }
     return -1;
 }
@@ -526,6 +661,12 @@ extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius,
         case PROMP_ENV_POINT_MOMENTUM:
             return hidden == 64 ? launch_rollout<PROMP_ENV_POINT_MOMENTUM, 64>(A, st)
                                 : launch_rollout<PROMP_ENV_POINT_MOMENTUM, 32>(A, st);
+        case PROMP_ENV_WALKER:
+            return hidden == 64 ? launch_rollout<PROMP_ENV_WALKER, 64>(A, st) : launch_rollout<PROMP_ENV_WALKER, 32>(A, st);
+        case PROMP_ENV_SWIMMER:
+            PROMP_REQUIRE(info != nullptr, "promp_rollout: the swimmer needs the info buffer [2,M,E,H]");
+            PROMP_REQUIRE(reward_type == 0, "promp_rollout: swimmer reward_type must be 0");
+            return hidden == 64 ? launch_rollout<PROMP_ENV_SWIMMER, 64>(A, st) : launch_rollout<PROMP_ENV_SWIMMER, 32>(A, st);
         case PROMP_ENV_POINT:
             set_error("promp_rollout: MetaPointEnv terminates early (variable-length paths); use the stepwise "
                       "sampler (promp_env_step) for it");
@@ -543,7 +684,8 @@ extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int
                                         const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
                                         const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs,
                                         float* act, float* mean, float* rew, uint8_t* done, float* log_std_out, void* stream) {
-    PROMP_REQUIRE(env_kind == PROMP_ENV_POINT, "promp_rollout_early_term: implemented for MetaPointEnv (env_kind %d given)", env_kind);
+    PROMP_REQUIRE(env_kind == PROMP_ENV_POINT || env_kind == PROMP_ENV_WALKER,
+                  "promp_rollout_early_term: implemented for MetaPointEnv and the walker (env_kind %d given)", env_kind);
     PROMP_REQUIRE(M > 0 && E > 0 && timeline_len > 0 && horizon > 0, "promp_rollout_early_term: sizes must be positive");
     PROMP_REQUIRE(M <= 65535, "promp_rollout_early_term: M=%d exceeds the grid.y limit 65535", M);
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out,
@@ -553,6 +695,8 @@ extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
                   nullptr, 1, horizon};
     cudaStream_t st = (cudaStream_t)stream;
+    if (env_kind == PROMP_ENV_WALKER)
+        return hidden == 64 ? launch_rollout<PROMP_ENV_WALKER, 64>(A, st) : launch_rollout<PROMP_ENV_WALKER, 32>(A, st);
     return hidden == 64 ? launch_rollout<PROMP_ENV_POINT, 64>(A, st) : launch_rollout<PROMP_ENV_POINT, 32>(A, st);
 }
 
@@ -597,6 +741,14 @@ extern "C" int promp_env_step(int env_kind, int reward_type, float sparse_radius
             env_step_kernel<PROMP_ENV_POINT_MOMENTUM><<<gs, bs, 0, st>>>(reward_type, sparse_radius, normalize_actions, n_env, H, state,
                                                                          ts, actions, task_params, reset_state, next_obs, rew, done, info);
             break;
+        case PROMP_ENV_WALKER:
+            env_step_kernel<PROMP_ENV_WALKER><<<gs, bs, 0, st>>>(reward_type, sparse_radius, normalize_actions, n_env, H, state, ts,
+                                                                 actions, task_params, reset_state, next_obs, rew, done, info);
+            break;
+        case PROMP_ENV_SWIMMER:
+            env_step_kernel<PROMP_ENV_SWIMMER><<<gs, bs, 0, st>>>(reward_type, sparse_radius, normalize_actions, n_env, H, state, ts,
+                                                                  actions, task_params, reset_state, next_obs, rew, done, info);
+            break;
         default:
             set_error("promp_env_step: unknown env_kind %d", env_kind);
             return PROMP_ERR_INVALID_ARG;
@@ -615,6 +767,8 @@ extern "C" int promp_env_observe(int env_kind, int n_env, const float* state, fl
         case PROMP_ENV_CHEETAH_DIR: env_observe_kernel<PROMP_ENV_CHEETAH_DIR><<<gs, bs, 0, st>>>(n_env, state, obs); break;
         case PROMP_ENV_POINT_WALLS: env_observe_kernel<PROMP_ENV_POINT_WALLS><<<gs, bs, 0, st>>>(n_env, state, obs); break;
         case PROMP_ENV_POINT_MOMENTUM: env_observe_kernel<PROMP_ENV_POINT_MOMENTUM><<<gs, bs, 0, st>>>(n_env, state, obs); break;
+        case PROMP_ENV_WALKER: env_observe_kernel<PROMP_ENV_WALKER><<<gs, bs, 0, st>>>(n_env, state, obs); break;
+        case PROMP_ENV_SWIMMER: env_observe_kernel<PROMP_ENV_SWIMMER><<<gs, bs, 0, st>>>(n_env, state, obs); break;
         default:
             set_error("promp_env_observe: unknown env_kind %d", env_kind);
             return PROMP_ERR_INVALID_ARG;

@@ -76,13 +76,14 @@ class MetaSampler(object):
 
     def _fused_ok(self):
         return (self.spec is not None and hasattr(self.policy, 'sampling_params')
-                and self.spec['env_kind'] != _lib.ENV_POINT and self.envs_per_task == self.batch_size)
+                and self.spec['env_kind'] not in _lib.EARLY_TERM_ENVS and self.envs_per_task == self.batch_size)
 
     def _fused_early_ok(self):
-        """Early-terminating MetaPointEnv through the fused kernel + device-side path table.  Opt-in via reset_mode='device':
-        in-kernel resets cannot follow the host numpy stream (their number is data-dependent), so reset_mode='numpy' keeps the
-        reference's step loop with host draws."""
-        return (self.spec is not None and hasattr(self.policy, 'sampling_params') and self.spec['env_kind'] == _lib.ENV_POINT
+        """Early-terminating envs (MetaPointEnv, the Walker2d surrogates) through the fused kernel + device-side path table.
+        Opt-in via reset_mode='device': in-kernel resets cannot follow the host numpy stream (their number is data-dependent),
+        so reset_mode='numpy' keeps the reference's step loop with host draws."""
+        return (self.spec is not None and hasattr(self.policy, 'sampling_params')
+                and self.spec['env_kind'] in _lib.EARLY_TERM_ENVS
                 and self.reset_mode == 'device' and self.envs_per_task == self.batch_size and self.envs_per_task <= 1024)
 
     def obtain_samples(self, log=False, log_prefix=''):
@@ -109,7 +110,7 @@ class MetaSampler(object):
         s = self.spec
         M, E, H = self.meta_batch_size, self.envs_per_task, self.max_path_length
         params, stride, clip = self.policy.sampling_params()
-        if s['env_kind'] == _lib.ENV_CHEETAH_DIR and phase.info is None:
+        if s['env_kind'] in _lib.INFO_ENVS and phase.info is None:
             keys = tuple(getattr(getattr(self.env, '_wrapped_env', self.env), 'info_keys', ('reward_run', 'reward_ctrl')))
             phase.info = torch.empty(len(keys), M, E * H, dtype=torch.float32, device=self.device)
             phase.info_keys = keys

@@ -34,7 +34,7 @@ class MetaDeviceEnvExecutor(object):
         self._rew = torch.zeros(self.n_envs, **f32)
         self._done = torch.zeros(self.n_envs, dtype=torch.uint8, device=self.device)
         inner_env = getattr(env, '_wrapped_env', env)
-        self.info_keys = tuple(getattr(inner_env, 'info_keys', ())) if self.spec['env_kind'] == _lib.ENV_CHEETAH_DIR else ()
+        self.info_keys = tuple(getattr(inner_env, 'info_keys', ())) if self.spec['env_kind'] in _lib.INFO_ENVS else ()
         self._info = torch.zeros(max(len(self.info_keys), 2), self.n_envs, **f32)
         self._dummy_reset = torch.zeros(self.n_envs, sd, **f32)
 
