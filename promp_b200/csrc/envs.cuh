@@ -10,32 +10,36 @@
 //                  Both restated on the CPU in oracle/locomotion_surrogates.py.
 //   NormalizedEnv: ref envs/normalized_env.py:109-117 (action affine map + clip; obs / reward
 //                  normalisation are off by default, :23-24, and out of scope).
+//
+// Each environment is one type (PointCorner, Point, PointWalls, PointMomentum, Cheetah, Walker, Swimmer) with
+//   KIND (PROMP_ENV_*), DO / DA (obs / action size), SD (floats of an init_state / final_state / reset_state row),
+//   TD (floats per task), NINFO (env_infos channels), NACC (rollout layer-1 accumulators: 2 where the env's registers
+//   leave no room for 4), ENDS_EARLY (the env reports `done` before the horizon);
+//   warp-resident state for rollout_kernel, one warp per env:
+//     load(init_state row, lane), reset(rng, step, tag, lane) (Philox draw), observe(shared obs line, lane),
+//     step(a, task, cfg, lane, info, info_stride, done) -> reward, store(final_state row, lane);
+//   one thread per env for env_step_kernel / env_observe_kernel:
+//     step_serial(st[SD], a, task, cfg, info, info_stride, done) -> reward, observe_serial(st, obs).
+// `info` is NULL or channel 0 of the env_infos record, channel c at info[c * info_stride].
 #pragma once
 #include "common.cuh"
 
 namespace promp {
 
-template <int KIND> struct EnvTraits;
-template <> struct EnvTraits<PROMP_ENV_POINT_CORNER> {
-    static constexpr int DO = 2, DA = 2, SD = 2, TD = 2, NINFO = 0;
+// step configuration every env receives
+struct EnvCfg {
+    int reward_type;
+    float radius;       // sparse reward radius
+    bool normalized;    // actions pass through the NormalizedEnv map
 };
-template <> struct EnvTraits<PROMP_ENV_POINT> {
-    static constexpr int DO = 2, DA = 2, SD = 2, TD = 1, NINFO = 0;
-};
-template <> struct EnvTraits<PROMP_ENV_CHEETAH_DIR> {
-    static constexpr int DO = 17, DA = 6, SD = 18, TD = 1, NINFO = 2;
-};
-template <> struct EnvTraits<PROMP_ENV_POINT_WALLS> {
-    static constexpr int DO = 2, DA = 2, SD = 2, TD = 6, NINFO = 0;       // task = goal, gap_1, gap_2
-};
-template <> struct EnvTraits<PROMP_ENV_POINT_MOMENTUM> {
-    static constexpr int DO = 4, DA = 2, SD = 4, TD = 2, NINFO = 0;       // state = obs = (pos, vel)
-};
-template <> struct EnvTraits<PROMP_ENV_WALKER> {
-    static constexpr int DO = 17, DA = 6, SD = 18, TD = 2, NINFO = 0;     // task = (direction | goal velocity, mode)
-};
-template <> struct EnvTraits<PROMP_ENV_SWIMMER> {
-    static constexpr int DO = 8, DA = 2, SD = 10, TD = 1, NINFO = 2;      // info = reward_fwd, reward_ctrl
+
+// Philox stream of one env slot: counter (env, ctr, stream_id low word, tag | stream_id bits 32-55), key = seed
+struct EnvRng {
+    uint32_t env, stream_lo, stream_hi;
+    uint64_t seed;
+    __device__ __forceinline__ void gen(uint32_t ctr, uint32_t tag, uint32_t (&r)[4]) const {
+        Philox::gen(env, ctr, stream_lo, tag | stream_hi, seed, r);
+    }
 };
 
 // NormalizedEnv.step action map, same evaluation order as the reference expression
@@ -45,17 +49,14 @@ __device__ __forceinline__ float normalized_action(float a, float lb, float ub) 
     return fminf(fmaxf(s, lb), ub);
 }
 // wrapped (normalize(env), every reference run script) or raw env (the reference's tests): the raw env receives the
-// policy action unchanged and applies only its own clip
-__device__ __forceinline__ float env_action(float a, float lb, float ub, bool normalized) {
-    return normalized ? normalized_action(a, lb, ub) : a;
+// policy action unchanged and applies only its own clip to [-lim, lim] (point_env_2d_corner.py:37; the identity after
+// the wrapper's clip)
+__device__ __forceinline__ float env_action(float a, float lim, bool normalized) {
+    const float e = normalized ? normalized_action(a, -lim, lim) : a;
+    return fminf(fmaxf(e, -lim), lim);
 }
-
-// ------------------------------------------------------------------ point corner
-struct PointCornerCfg {
-    int reward_type;
-    float radius;
-    bool normalized;
-};
+// MuJoCo envs: the raw env's ctrlrange clips the torque to [-1, 1] inside the simulator
+__device__ __forceinline__ float ctrl_action(float a, bool normalized) { return env_action(a, 1.f, normalized); }
 
 // sqrt.approx (MUFU.RSQ-based, max relative error 2^-23 per the PTX ISA, i.e. within 1 ulp of sqrtf) without sqrtf's
 // fix-up sequence and slow-path branch: the sparse reward needs five to six distances per env step and the branches
@@ -70,98 +71,222 @@ __device__ __forceinline__ float dist2d(float x, float y, float gx, float gy) {
     return sqrt_fast(dx * dx + dy * dy);
 }
 
-// s (in/out): state; (ax, ay): policy-space action.  Returns reward.
-__device__ __forceinline__ float point_corner_step(float& sx, float& sy, float ax, float ay, float gx, float gy,
-                                                   const PointCornerCfg& cfg) {
-    const float lim = 0.2f;
-    float ex = env_action(ax, -lim, lim, cfg.normalized), ey = env_action(ay, -lim, lim, cfg.normalized);
-    // env-side clip (point_env_2d_corner.py:37); the identity after the wrapper's clip
-    ex = fminf(fmaxf(ex, -lim), lim);
-    ey = fminf(fmaxf(ey, -lim), lim);
-    float px = sx, py = sy;
-    sx = px + ex;
-    sy = py + ey;
-    float r;
-    if (cfg.reward_type == PROMP_REWARD_DENSE) {
-        r = -dist2d(sx, sy, gx, gy);
-    } else if (cfg.reward_type == PROMP_REWARD_DENSE_SQUARED) {
-        float g = dist2d(sx, sy, gx, gy);
-        r = -(g * g);
-    } else {
-        // sparse (:68-75): 0 inside the L1 radius; progress toward the goal iff the goal is the nearest corner
-        float d0 = dist2d(sx, sy, -2.f, -2.f), d1 = dist2d(sx, sy, 2.f, -2.f);
-        float d2 = dist2d(sx, sy, -2.f, 2.f), d3 = dist2d(sx, sy, 2.f, 2.f);
-        float dmin = fminf(fminf(d0, d1), fminf(d2, d3));
-        float g;   // take the goal distance from the same four values when the goal is a corner (exact ==)
-        if (gx == -2.f && gy == -2.f) g = d0;
-        else if (gx == 2.f && gy == -2.f) g = d1;
-        else if (gx == -2.f && gy == 2.f) g = d2;
-        else if (gx == 2.f && gy == 2.f) g = d3;
-        else g = dist2d(sx, sy, gx, gy);
-        r = 0.f;
-        if (!(fabsf(sx) + fabsf(sy) < cfg.radius) && g == dmin) r = dist2d(px, py, gx, gy) - g;
+// State that every lane of the env's warp holds and advances identically: the warp step is the serial step on that copy
+// and lane 0 writes what leaves the warp.
+template <class Env, int SD>
+struct Replicated {
+    float s[SD];
+    __device__ __forceinline__ void load(const float* s0, int) {
+#pragma unroll
+        for (int k = 0; k < SD; ++k) s[k] = s0[k];
     }
-    return r;
-}
+    __device__ __forceinline__ void store(float* fs, int lane) const {
+        if (lane == 0)
+#pragma unroll
+            for (int k = 0; k < SD; ++k) fs[k] = s[k];
+    }
+    __device__ __forceinline__ void observe(float* obs, int lane) const {
+        if (lane == 0) Env::observe_serial(s, obs);
+    }
+    __device__ __forceinline__ float step(const float* a, const float* task, const EnvCfg& cfg, int lane, float* info,
+                                          int info_stride, bool& done) {
+        return Env::step_serial(s, a, task, cfg, lane == 0 ? info : nullptr, info_stride, done);
+    }
+};
+
+// point envs: obs = state = position (++ velocity for the momentum env).  reset (point_env_2d_corner.py:50 /
+// point_env_2d.py:34 / point_env_2d_momentum.py:52): position U(-RESET_LIM, RESET_LIM)^2, velocity U(-.1,.1)^2, from
+// counter `step`.
+template <class Env, int SD>
+struct PointState : Replicated<Env, SD> {
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int) {
+        uint32_t r[4];
+        rng.gen(step, tag, r);
+        const float lim = Env::RESET_LIM;
+        this->s[0] = -lim + 2.f * lim * u01(r[0]);
+        this->s[1] = -lim + 2.f * lim * u01(r[1]);
+        if constexpr (SD == 4) this->s[2] = -0.1f + 0.2f * u01(r[2]), this->s[3] = -0.1f + 0.2f * u01(r[3]);
+    }
+    static __device__ __forceinline__ void observe_serial(const float* st, float* obs) {
+#pragma unroll
+        for (int k = 0; k < SD; ++k) obs[k] = st[k];
+    }
+};
+
+// ------------------------------------------------------------------ point corner
+struct PointCorner : PointState<PointCorner, 2> {
+    static constexpr int KIND = PROMP_ENV_POINT_CORNER, DO = 2, DA = 2, SD = 2, TD = 2, NINFO = 0, NACC = 4;
+    static constexpr bool ENDS_EARLY = false;
+    static constexpr float RESET_LIM = 0.2f;
+    // s (in/out): state; a: policy-space action; task: goal.  Returns reward.
+    static __device__ __forceinline__ float step_serial(float (&s)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float*, int, bool&) {
+        float &sx = s[0], &sy = s[1];
+        const float gx = task[0], gy = task[1];
+        const float ex = env_action(a[0], 0.2f, cfg.normalized), ey = env_action(a[1], 0.2f, cfg.normalized);
+        float px = sx, py = sy;
+        sx = px + ex;
+        sy = py + ey;
+        float r;
+        if (cfg.reward_type == PROMP_REWARD_DENSE) {
+            r = -dist2d(sx, sy, gx, gy);
+        } else if (cfg.reward_type == PROMP_REWARD_DENSE_SQUARED) {
+            float g = dist2d(sx, sy, gx, gy);
+            r = -(g * g);
+        } else {
+            // sparse (:68-75): 0 inside the L1 radius; progress toward the goal iff the goal is the nearest corner
+            float d0 = dist2d(sx, sy, -2.f, -2.f), d1 = dist2d(sx, sy, 2.f, -2.f);
+            float d2 = dist2d(sx, sy, -2.f, 2.f), d3 = dist2d(sx, sy, 2.f, 2.f);
+            float dmin = fminf(fminf(d0, d1), fminf(d2, d3));
+            float g;   // take the goal distance from the same four values when the goal is a corner (exact ==)
+            if (gx == -2.f && gy == -2.f) g = d0;
+            else if (gx == 2.f && gy == -2.f) g = d1;
+            else if (gx == -2.f && gy == 2.f) g = d2;
+            else if (gx == 2.f && gy == 2.f) g = d3;
+            else g = dist2d(sx, sy, gx, gy);
+            r = 0.f;
+            if (!(fabsf(sx) + fabsf(sy) < cfg.radius) && g == dmin) r = dist2d(px, py, gx, gy) - g;
+        }
+        return r;
+    }
+};
 
 // ------------------------------------------------------------------ point (origin goal, early done)
-__device__ __forceinline__ float point_step(float& sx, float& sy, float ax, float ay, bool& done, bool normalized) {
-    const float lim = 0.1f;
-    float ex = env_action(ax, -lim, lim, normalized), ey = env_action(ay, -lim, lim, normalized);
-    ex = fminf(fmaxf(ex, -lim), lim);
-    ey = fminf(fmaxf(ey, -lim), lim);
-    sx += ex;
-    sy += ey;
-    done = (fabsf(sx) < 0.01f) && (fabsf(sy) < 0.01f);
-    return -sqrt_fast(sx * sx + sy * sy);
-}
+struct Point : PointState<Point, 2> {
+    static constexpr int KIND = PROMP_ENV_POINT, DO = 2, DA = 2, SD = 2, TD = 1, NINFO = 0, NACC = 4;
+    static constexpr bool ENDS_EARLY = true;
+    static constexpr float RESET_LIM = 2.0f;
+    static __device__ __forceinline__ float step_serial(float (&s)[SD], const float* a, const float*, const EnvCfg& cfg, float*,
+                                                        int, bool& done) {
+        float &sx = s[0], &sy = s[1];
+        const float ex = env_action(a[0], 0.1f, cfg.normalized), ey = env_action(a[1], 0.1f, cfg.normalized);
+        sx += ex;
+        sy += ey;
+        done = (fabsf(sx) < 0.01f) && (fabsf(sy) < 0.01f);
+        return -sqrt_fast(sx * sx + sy * sy);
+    }
+};
 
 // ------------------------------------------------------------------ point walls (ref point_env_2d_walls.py:22-51)
 // s' = s + clip(a, +-0.2); the reward is taken at s' BEFORE the wall logic (:37-39); crossing the unit circle outside
 // gap_1 (distance > 1 from the gap centre) projects s' back to just inside radius 1, crossing the radius-2 circle
 // outside gap_2 to just inside radius 2 (:40-49).  reward_type dense / dense_squared (the reference's 'sparse' branch
 // returns None outside the radius and cannot be sampled).
-__device__ __forceinline__ float point_walls_step(float& sx, float& sy, float ax, float ay, const float* task, int reward_type,
-                                                  bool normalized) {
-    const float lim = 0.2f;
-    float ex = env_action(ax, -lim, lim, normalized), ey = env_action(ay, -lim, lim, normalized);
-    ex = fminf(fmaxf(ex, -lim), lim);
-    ey = fminf(fmaxf(ey, -lim), lim);
-    const float px = sx, py = sy;
-    float nx = px + ex, ny = py + ey;
-    const float g = dist2d(nx, ny, task[0], task[1]);
-    const float r = (reward_type == PROMP_REWARD_DENSE_SQUARED) ? -(g * g) : -g;
-    const float pn = sqrt_fast(px * px + py * py), nn = sqrt_fast(nx * nx + ny * ny);
-    if (pn < 1.f && nn > 1.f) {
-        if (dist2d(nx, ny, task[2], task[3]) > 1.f) {
-            const float inv = 1.f / (nn + 1e-6f);
-            nx *= inv, ny *= inv;
+struct PointWalls : PointState<PointWalls, 2> {
+    static constexpr int KIND = PROMP_ENV_POINT_WALLS, DO = 2, DA = 2, SD = 2, TD = 6, NINFO = 0, NACC = 4;   // task = goal, gap_1, gap_2
+    static constexpr bool ENDS_EARLY = false;
+    static constexpr float RESET_LIM = 0.2f;
+    static __device__ __forceinline__ float step_serial(float (&s)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float*, int, bool&) {
+        float &sx = s[0], &sy = s[1];
+        const float ex = env_action(a[0], 0.2f, cfg.normalized), ey = env_action(a[1], 0.2f, cfg.normalized);
+        const float px = sx, py = sy;
+        float nx = px + ex, ny = py + ey;
+        const float g = dist2d(nx, ny, task[0], task[1]);
+        const float r = (cfg.reward_type == PROMP_REWARD_DENSE_SQUARED) ? -(g * g) : -g;
+        const float pn = sqrt_fast(px * px + py * py), nn = sqrt_fast(nx * nx + ny * ny);
+        if (pn < 1.f && nn > 1.f) {
+            if (dist2d(nx, ny, task[2], task[3]) > 1.f) {
+                const float inv = 1.f / (nn + 1e-6f);
+                nx *= inv, ny *= inv;
+            }
+        } else if (pn < 2.f && nn > 2.f) {
+            if (dist2d(nx, ny, task[4], task[5]) > 1.f) {
+                const float inv = 1.f / (nn * 0.5f + 1e-6f);
+                nx *= inv, ny *= inv;
+            }
         }
-    } else if (pn < 2.f && nn > 2.f) {
-        if (dist2d(nx, ny, task[4], task[5]) > 1.f) {
-            const float inv = 1.f / (nn * 0.5f + 1e-6f);
-            nx *= inv, ny *= inv;
-        }
+        sx = nx, sy = ny;
+        return r;
     }
-    sx = nx, sy = ny;
-    return r;
-}
+};
 
 // ------------------------------------------------------------------ point momentum (ref point_env_2d_momentum.py:22-42, 58-68)
 // v' = v + clip(a, +-0.1); s' = s + v'; obs = (s', v'); reward at s': sparse (default) = max(radius - |s' - goal|, 0)
-__device__ __forceinline__ float point_momentum_step(float& sx, float& sy, float& vx, float& vy, float ax, float ay, float gx,
-                                                     float gy, const PointCornerCfg& cfg) {
-    const float lim = 0.1f;
-    float ex = env_action(ax, -lim, lim, cfg.normalized), ey = env_action(ay, -lim, lim, cfg.normalized);
-    ex = fminf(fmaxf(ex, -lim), lim);
-    ey = fminf(fmaxf(ey, -lim), lim);
-    vx += ex, vy += ey;
-    sx += vx, sy += vy;
-    const float g = dist2d(sx, sy, gx, gy);
-    if (cfg.reward_type == PROMP_REWARD_DENSE) return -g;
-    if (cfg.reward_type == PROMP_REWARD_DENSE_SQUARED) return -(g * g);
-    return fmaxf(cfg.radius - g, 0.f);
-}
+struct PointMomentum : PointState<PointMomentum, 4> {
+    static constexpr int KIND = PROMP_ENV_POINT_MOMENTUM, DO = 4, DA = 2, SD = 4, TD = 2, NINFO = 0, NACC = 4;   // state = (pos, vel)
+    static constexpr bool ENDS_EARLY = false;
+    static constexpr float RESET_LIM = 0.2f;
+    static __device__ __forceinline__ float step_serial(float (&s)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float*, int, bool&) {
+        float &sx = s[0], &sy = s[1], &vx = s[2], &vy = s[3];
+        const float gx = task[0], gy = task[1];
+        const float ex = env_action(a[0], 0.1f, cfg.normalized), ey = env_action(a[1], 0.1f, cfg.normalized);
+        vx += ex, vy += ey;
+        sx += vx, sy += vy;
+        const float g = dist2d(sx, sy, gx, gy);
+        if (cfg.reward_type == PROMP_REWARD_DENSE) return -g;
+        if (cfg.reward_type == PROMP_REWARD_DENSE_SQUARED) return -(g * g);
+        return fmaxf(cfg.radius - g, 0.f);
+    }
+};
+
+// ------------------------------------------------------------------ planar 9-DoF state (cheetah, walker)
+// state row = qpos[9] ++ qvel[9], qpos = root (x, z, pitch) ++ joint[6].  In the warp, lane j < 6 owns joint j (q, qd) and
+// the six root floats (x, z, pitch, xd, zd, pd) are replicated in every lane.  obs = qpos[1:] ++ qvel
+// (half_cheetah_rand_direc.py:43-47); CLIP_VEL: the walker's obs clips qvel to [-10, 10] (walker2d_rand_*.py:42-45).
+template <bool CLIP_VEL>
+struct Planar9 {
+    float q, qd, root[6];
+
+    static __device__ __forceinline__ float obs_vel(float v) { return CLIP_VEL ? fminf(fmaxf(v, -10.0f), 10.0f) : v; }
+
+    __device__ __forceinline__ void load(const float* s0, int lane) {
+        const int jl = lane & 7;
+        root[0] = s0[0]; root[1] = s0[1]; root[2] = s0[2];
+        root[3] = s0[9]; root[4] = s0[10]; root[5] = s0[11];
+        q = jl < 6 ? s0[3 + jl] : 0.f;
+        qd = jl < 6 ? s0[12 + jl] : 0.f;
+    }
+    __device__ __forceinline__ void store(float* fs, int lane) const {
+        if (lane == 0) {
+            fs[0] = root[0]; fs[1] = root[1]; fs[2] = root[2];
+            fs[9] = root[3]; fs[10] = root[4]; fs[11] = root[5];
+        }
+        if (lane < 6) {
+            fs[3 + lane] = q;
+            fs[12 + lane] = qd;
+        }
+    }
+    __device__ __forceinline__ void observe(float* obs, int lane) const {
+        if (lane == 0) {
+            obs[0] = root[1]; obs[1] = root[2];
+            obs[8] = obs_vel(root[3]); obs[9] = obs_vel(root[4]); obs[10] = obs_vel(root[5]);
+        }
+        if (lane < 6) {
+            obs[2 + lane] = q;
+            obs[11 + lane] = obs_vel(qd);
+        }
+    }
+    static __device__ __forceinline__ void observe_serial(const float* st, float* obs) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) obs[k] = st[1 + k];
+#pragma unroll
+        for (int k = 0; k < 9; ++k) obs[8 + k] = obs_vel(st[9 + k]);
+    }
+    // spreads a reset draw over the warp: lane i < 9 holds coordinate i of qpos (pos) and of qvel (vel)
+    __device__ __forceinline__ void spread(float pos, float vel, int lane) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            root[i] = __shfl_sync(0xffffffffu, pos, i);
+            root[3 + i] = __shfl_sync(0xffffffffu, vel, i);
+        }
+        const int jl = lane & 7;
+        const float qq = __shfl_sync(0xffffffffu, pos, 3 + (jl < 6 ? jl : 0));
+        const float qv = __shfl_sync(0xffffffffu, vel, 3 + (jl < 6 ? jl : 0));
+        q = jl < 6 ? qq : 0.f;
+        qd = jl < 6 ? qv : 0.f;
+    }
+    // this lane's joint torque: the clipped control of action lane & 7, 0 on lanes 6 and 7
+    static __device__ __forceinline__ float joint_ctrl(const float* a, int lane, bool normalized) {
+        float al = 0.f;
+        const int jl = lane & 7;
+#pragma unroll
+        for (int d = 0; d < 6; ++d)
+            if (jl == d) al = a[d];
+        return jl < 6 ? ctrl_action(al, normalized) : 0.f;
+    }
+};
 
 // ------------------------------------------------------------------ cheetah surrogate
 namespace cheetah {
@@ -279,6 +404,54 @@ __device__ __forceinline__ void step_warp(const JointConst& jc, float u, float& 
 }
 }  // namespace cheetah
 
+// task = direction (reward_type 0, RandDirec) or goal velocity (reward_type 1, RandVel);
+// info = reward_run, reward_ctrl (++ forward_vel for RandVel)
+struct Cheetah : Planar9<false> {
+    static constexpr int KIND = PROMP_ENV_CHEETAH_DIR, DO = 17, DA = 6, SD = 18, TD = 1, NINFO = 2, NACC = 2;
+    static constexpr bool ENDS_EARLY = false;
+    cheetah::JointConst jc = cheetah::joint_const(threadIdx.x & 7);   // this lane's joint (lane & 7)
+
+    // reset_model (half_cheetah_rand_direc.py:49-53): qpos = U(-.1,.1)^9, qvel = .1*N(0,1)^9; lane i < 9 draws coordinate
+    // i from counter (step << 4) + i
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane) {
+        float pos = 0.f, vel = 0.f;
+        if (lane < 9) {
+            uint32_t r[4];
+            rng.gen((step << 4) + (uint32_t)lane, tag, r);
+            pos = -0.1f + 0.2f * u01(r[0]);
+            float z0, z1;
+            box_muller(r[1], r[2], z0, z1);
+            vel = 0.1f * z0;
+        }
+        spread(pos, vel, lane);
+    }
+    __device__ __forceinline__ float step(const float* a, const float* task, const EnvCfg& cfg, int lane, float* info,
+                                          int info_stride, bool&) {
+        float r, r_run, r_ctrl, fwd_vel;
+        cheetah::step_warp(jc, joint_ctrl(a, lane, cfg.normalized), q, qd, root, task[0], cfg.reward_type, r, r_run, r_ctrl,
+                           fwd_vel);
+        if (lane == 0) {
+            info[0] = r_run;
+            info[info_stride] = r_ctrl;
+            info[2 * info_stride] = fwd_vel;
+        }
+        return r;
+    }
+    static __device__ __forceinline__ float step_serial(float (&st)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float* info, int info_stride, bool&) {
+        float u[DA], r, r_run, r_ctrl, fwd_vel;
+#pragma unroll
+        for (int k = 0; k < DA; ++k) u[k] = ctrl_action(a[k], cfg.normalized);
+        cheetah::step_serial(st, u, task[0], cfg.reward_type, r, r_run, r_ctrl, fwd_vel);
+        if (info) {
+            info[0] = r_run;
+            info[info_stride] = r_ctrl;
+            if (cfg.reward_type == 1) info[2 * info_stride] = fwd_vel;
+        }
+        return r;
+    }
+};
+
 // ------------------------------------------------------------------ walker2d surrogate
 // MuJoCo-free Walker2DRandVel / Walker2DRandDirec: obs / reward / done / reset follow ref envs/mujoco_envs/
 // walker2d_rand_vel.py:32-55 and walker2d_rand_direc.py:32-55; the dynamics are defined in DESIGN.md §3.4 and restated
@@ -308,8 +481,6 @@ __device__ __forceinline__ JointConst joint_const(int j) {
 __device__ __forceinline__ bool is_done(float z, float ang) {
     return !(z > 0.8f && z < 2.0f && ang > -1.0f && ang < 1.0f);
 }
-// obs clips qvel to [-10, 10] (walker2d_rand_*.py:42-45)
-__device__ __forceinline__ float clip_vel(float v) { return fminf(fmaxf(v, -10.0f), 10.0f); }
 
 // mode 0: RandDirec, reward = dir * fwd_vel + 1 - 1e-3 |u|^2;  mode 1: RandVel, reward = -|fwd_vel - goal| + 15 - 1e-3 |u|^2
 __device__ __forceinline__ float reward(float fwd_vel, float su, float task, int mode) {
@@ -397,6 +568,44 @@ __device__ __forceinline__ void step_warp(const JointConst& jc, float u, float& 
 }
 }  // namespace walker
 
+// task = (direction | goal velocity, reward mode)
+struct Walker : Planar9<true> {
+    static constexpr int KIND = PROMP_ENV_WALKER, DO = 17, DA = 6, SD = 18, TD = 2, NINFO = 0, NACC = 2;
+    static constexpr bool ENDS_EARLY = true;
+    walker::JointConst jc = walker::joint_const(threadIdx.x & 7);     // this lane's joint (lane & 7)
+
+    // reset_model (walker2d_rand_*.py:47-52): qpos = init_qpos + U(-.005,.005)^9 (init_qpos z = 1.25, all else 0),
+    // qvel = U(-.005,.005)^9; lane i < 9 draws coordinate i from counter (step << 4) + i
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane) {
+        float pos = 0.f, vel = 0.f;
+        if (lane < 9) {
+            uint32_t r[4];
+            rng.gen((step << 4) + (uint32_t)lane, tag, r);
+            pos = -0.005f + 0.01f * u01(r[0]);
+            vel = -0.005f + 0.01f * u01(r[1]);
+        }
+        spread(pos, vel, lane);
+        root[1] += 1.25f;
+    }
+    // the root is replicated, so `done` is warp-uniform
+    __device__ __forceinline__ float step(const float* a, const float* task, const EnvCfg& cfg, int lane, float*, int,
+                                          bool& done) {
+        float r, fwd_vel;
+        walker::step_warp(jc, joint_ctrl(a, lane, cfg.normalized), q, qd, root, task[0], task[TD - 1] != 0.f, r, fwd_vel);
+        done = walker::is_done(root[1], root[2]);
+        return r;
+    }
+    static __device__ __forceinline__ float step_serial(float (&st)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float*, int, bool& done) {
+        float u[DA], r, fwd_vel;
+#pragma unroll
+        for (int k = 0; k < DA; ++k) u[k] = ctrl_action(a[k], cfg.normalized);
+        walker::step_serial(st, u, task[0], task[TD - 1] != 0.f, r, fwd_vel);
+        done = walker::is_done(st[1], st[2]);
+        return r;
+    }
+};
+
 // ------------------------------------------------------------------ swimmer surrogate
 // MuJoCo-free SwimmerRandVel: obs / reward / reset follow ref envs/mujoco_envs/swimmer_rand_vel.py:30-50 (reward_fwd =
 // |fwd_vel - goal| with the reference's sign), the dynamics are defined in DESIGN.md §3.4 (CPU: oracle/
@@ -436,5 +645,39 @@ __device__ __forceinline__ void step(float (&st)[10], float u0, float u1, float 
     rew = r_fwd + r_ctrl;
 }
 }  // namespace swimmer
+
+// task = goal velocity; info = reward_fwd, reward_ctrl
+struct Swimmer : Replicated<Swimmer, 10> {
+    static constexpr int KIND = PROMP_ENV_SWIMMER, DO = 8, DA = 2, SD = 10, TD = 1, NINFO = 2, NACC = 4;
+    static constexpr bool ENDS_EARLY = false;
+
+    // reset_model (swimmer_rand_vel.py:41-46): qpos = U(-.1,.1)^5, qvel = U(-.1,.1)^5 from counters (step << 4) + 0..2
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int) {
+#pragma unroll
+        for (int blk = 0; blk < 3; ++blk) {
+            uint32_t r[4];
+            rng.gen((step << 4) + (uint32_t)blk, tag, r);
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+                if (blk * 4 + i < SD) s[blk * 4 + i] = -0.1f + 0.2f * u01(r[i]);
+        }
+    }
+    static __device__ __forceinline__ float step_serial(float (&st)[SD], const float* a, const float* task, const EnvCfg& cfg,
+                                                        float* info, int info_stride, bool&) {
+        const float u0 = ctrl_action(a[0], cfg.normalized), u1 = ctrl_action(a[1], cfg.normalized);
+        float r, r_fwd, r_ctrl;
+        swimmer::step(st, u0, u1, task[0], r, r_fwd, r_ctrl);
+        if (info) {
+            info[0] = r_fwd;
+            info[info_stride] = r_ctrl;
+        }
+        return r;
+    }
+    // obs = qpos[2:] ++ qvel (swimmer_rand_vel.py:37-40)
+    static __device__ __forceinline__ void observe_serial(const float* st, float* obs) {
+#pragma unroll
+        for (int k = 0; k < DO; ++k) obs[k] = st[2 + k];
+    }
+};
 
 }  // namespace promp

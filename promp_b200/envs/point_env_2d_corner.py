@@ -1,5 +1,5 @@
 """MetaPointEnvCorner (ref: meta_policy_search/envs/point_envs/point_env_2d_corner.py:7-93).
-Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: point_corner_step)."""
+Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: PointCorner)."""
 import numpy as np
 
 from promp_b200 import _lib

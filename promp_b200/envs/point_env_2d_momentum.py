@@ -1,6 +1,6 @@
 """MetaPointEnvMomentum (ref: meta_policy_search/envs/point_envs/point_env_2d_momentum.py:7-88): the clipped action is an
 acceleration, obs = (position, velocity), sparse reward = max(radius - goal distance, 0).
-Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: point_momentum_step)."""
+Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: PointMomentum)."""
 import numpy as np
 
 from promp_b200 import _lib

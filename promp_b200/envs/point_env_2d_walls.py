@@ -1,6 +1,6 @@
 """MetaPointEnvWalls (ref: meta_policy_search/envs/point_envs/point_env_2d_walls.py:7-117): two circular walls of radius 1
 and 2 around the origin, each passable only within distance 1 of its gap centre; tasks = goal corner + the two gaps.
-Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: point_walls_step)."""
+Dynamics/reward run on the GPU (promp_b200/csrc/envs.cuh: PointWalls)."""
 import numpy as np
 
 from promp_b200 import _lib

@@ -45,7 +45,7 @@ def main():
             run()
         lib.promp_debug_rollout_clocks(buf, 1)
         names = ['prologue (weights -> registers, reset)', 'noise chunk + flush chunk', 'layer 0 + tanh + stage obs + syncwarp', 'layer 1 (64x64, registers)',
-                 'tanh + layer 2 + warp_sum', 'sample + stage act/mean', 'env step', 'syncwarp + write_obs + syncwarp']
+                 'tanh + layer 2 + warp_sum', 'sample + stage act/mean', 'env step', 'syncwarp + observe + syncwarp']
         H = sampler.max_path_length
         tot = sum(buf[i] for i in range(8))
         print('  warp 0 clocks per launch %.0f (%.0f per env step):' % (tot / n, tot / n / H))
