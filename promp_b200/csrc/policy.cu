@@ -9,158 +9,10 @@
 // crosses a task boundary (or ends) it flushes them to a per-(CTA,task) partial slot, and the last
 // segment of each task to arrive (atomic ticket) reduces that task's slots in CTA order -> bitwise
 // run-to-run deterministic sums.  These kernels are fp32-FMA bound (AI ~ 10^2..10^3 FLOP/B).
-#include <stddef.h>
 #include <string.h>
-#include "mlp_tile.cuh"
+#include "policy_tc.cuh"
 
 namespace promp {
-
-template <int DO>
-struct DOPad {
-    static constexpr int V = (DO + 3) / 4 * 4;
-};
-
-constexpr int PSTAT = 4;   // per-partial trailing stats: sum obj, sum kl, sum ratio, unused
-
-struct PolicyArgs {
-    int M, N;
-    const float* params;
-    int64_t param_stride;
-    const float *obs, *act, *adv, *old_mean, *old_ls;
-    int ls_per_sample;
-    int obj_kind;
-    float obj_scale, clip_eps, kl_coeff;
-    int clip_log_std;
-    float min_log_std;
-    int obs_dim;         // logical observation / action sizes; read only by the padded instantiations (IsBucket below).  Both
-                         // sit in what was alignment padding: the struct's size and field offsets, and so the parameter
-                         // layout of every kernel taking PolicyArgs or ChainArgs, are unchanged.
-    // grad kernel
-    float* grad;
-    float* out_params;
-    float sgd_lr;
-    int act_dim;
-    // hvp kernel
-    const float* vec;
-    float* out;
-    float inner_lr;
-    float* stats;
-    float* partial;      // [grid][kmax][P + PSTAT] per-(CTA, task-segment) partial sums
-    int* counters;       // [M], zero on entry, left zero on exit
-    int q;               // tiles per CTA
-    int kmax;            // max task segments per CTA
-    const int32_t* n_valid;   // [M] valid samples per task (rows >= n_valid[m] are padding) or nullptr = N everywhere
-    // Re-use of an identical earlier launch (grad kernels only): the inner pass of the first Adam epoch repeats MAMLAlgo._adapt
-    // (same theta, same phase-0 data, same outputs) unless the reported-log_std clip of the step-0 graph is active.
-    //   producer side: unclipped_out = 1 iff every log_std component >= min_log_std, theta_copy_out = the parameters it used
-    //   consumer side: the whole grid returns at once if *skip_flag != 0 and params == skip_theta bit for bit (its outputs
-    //                  alias the producer's, which are then already correct)
-    const int* skip_flag;
-    const float* skip_theta;
-    int* unclipped_out;
-    float* theta_copy_out;
-    // optional device-resident multiplier of kl_coeff (ProMP's adaptive inner-KL coefficient lives on the device so that an
-    // iteration has no host decision: promp_adapt_kl_coeff updates it between launches)
-    const float* kl_coeff_ptr;
-};
-static_assert(sizeof(PolicyArgs) == 224 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120,
-              "PolicyArgs layout");
-__device__ __forceinline__ float kl_coeff_eff(const PolicyArgs& A) {
-    return A.kl_coeff_ptr ? A.kl_coeff * __ldcg(A.kl_coeff_ptr) : A.kl_coeff;
-}
-
-// Padded instantiations ("buckets"): compiled at the caps (DO, DA) of the zero-padded parameter layout of
-// promp_policy_layout, they take the logical observation / action sizes from PolicyArgs at run time.  Observations are
-// read with row stride obs_dim and zero-filled above it; action-side data (act, old_mean, old_log_std, mean) with row
-// stride act_dim, entries d >= act_dim never touched; the Gaussian head masks d >= act_dim out of every sum and gradient.
-// Pad rows of W0, pad columns of W2 and pad entries of b2 / log_std therefore get gradients and HVPs of exactly zero.
-// Whether a (DO, DA) instantiation is a bucket is known at compile time, so the exact instantiations compile to the code
-// they had.  The caps: obs_dim 1..8 -> 8, 9..19 -> 20; act_dim 1..2 -> 2, 3..8 -> 8 (even: P % 4 == 0).
-template <int DO, int DA>
-struct IsBucket {
-    static constexpr bool value = (DO == 8 || DO == 20) && (DA == 2 || DA == 8);
-};
-template <int DO, int DA>
-__device__ __forceinline__ int obs_dim_of(const PolicyArgs& A) {
-    if constexpr (IsBucket<DO, DA>::value) return A.obs_dim;
-    return DO;
-}
-template <int DO, int DA>
-__device__ __forceinline__ int act_dim_of(const PolicyArgs& A) {
-    if constexpr (IsBucket<DO, DA>::value) return A.act_dim;
-    return DA;
-}
-
-// consumer / producer halves of the launch re-use protocol above; returns true if the calling CTA must exit
-template <int P, int LS, int DA>
-__device__ __forceinline__ bool grad_reuse_prologue(const PolicyArgs& A) {
-    if (A.skip_flag) {
-        bool same = *reinterpret_cast<const volatile int*>(A.skip_flag) != 0;
-        for (int i = threadIdx.x; i < P && same; i += blockDim.x)
-            same = __float_as_uint(__ldcg(A.params + i)) == __float_as_uint(__ldcg(A.skip_theta + i));
-        if (__syncthreads_and(same ? 1 : 0)) return true;
-    }
-    if (A.unclipped_out && blockIdx.x == 0) {
-        if (threadIdx.x == 0) {
-            int ok = 1;
-            for (int d = 0; d < DA; ++d)
-                if (!(__ldcg(A.params + LS + d) >= A.min_log_std)) ok = 0;
-            *A.unclipped_out = ok;
-        }
-        for (int i = threadIdx.x; i < P; i += blockDim.x) A.theta_copy_out[i] = __ldcg(A.params + i);
-    }
-    return false;
-}
-
-// Tile-range bookkeeping shared by both kernels.
-struct TileSched {
-    int ntiles, T, q, g_lo, g_hi;
-    __device__ __forceinline__ TileSched(int M, int N, int q_, int tb = TB) {
-        ntiles = (N + tb - 1) / tb;
-        T = M * ntiles;
-        q = q_;
-        g_lo = blockIdx.x * q;
-        g_hi = min(g_lo + q, T);
-    }
-    __device__ __forceinline__ int first_task(int c) const { return (c * q) / ntiles; }
-    __device__ __forceinline__ int cta_lo(int m) const { return (m * ntiles) / q; }
-    __device__ __forceinline__ int cta_hi(int m) const { return ((m + 1) * ntiles - 1) / q; }
-};
-
-
-// Sum one float4 column of a task's partial slots over its CTA segments [c_lo, c_hi] in CTA order, with eight
-// independent L2 loads in flight (the naive dependent loop costs ~50 us of serial latency at the kernel tail).
-__device__ __forceinline__ float4 reduce_segments4(const float* partial, const TileSched& ts, int kmax, int pstride, int m,
-                                                   int c_lo, int c_hi, int p) {
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int c0 = c_lo; c0 <= c_hi; c0 += 8) {
-        float4 v[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            const int c = c0 + u;
-            v[u] = (c <= c_hi) ? __ldcg(reinterpret_cast<const float4*>(
-                                     partial + ((int64_t)c * kmax + (m - ts.first_task(c))) * pstride + p))
-                               : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) s.x += v[u].x, s.y += v[u].y, s.z += v[u].z, s.w += v[u].w;
-    }
-    return s;
-}
-
-template <int DO, int DA, int HID>
-__device__ __forceinline__ void load_head_consts(const float* P, int clip, float min_ls, HeadIn<DA>& hin, int da = DA) {
-    using L = PLayout<DO, DA, HID>;
-#pragma unroll
-    for (int d = 0; d < DA; ++d) {
-        const float raw = P[L::LS + d];
-        const bool clipped = clip && (raw < min_ls);      // tf.maximum: gradient goes to x when x >= y
-        hin.ls[d] = clipped ? min_ls : raw;
-        hin.ls_mask[d] = (clipped || d >= da) ? 0.f : 1.f;      // padding (d >= da) gets no log_std gradient either
-        hin.sig[d] = expf(hin.ls[d]);
-    }
-    head_in_finish<DA>(hin, da);
-}
 
 // -------------------------------------------------------------------------------------------------
 // Thread roles inside a 256-thread CTA working on a 64-sample tile:
@@ -193,9 +45,6 @@ struct GradSmem {
     int last;
 };
 
-// Combine per-thread partial sums through shared memory: out[idx] = sum_p scratch[p][idx], idx < n.
-// `mine(i)` yields this thread's partial for its i-th element; thread `tid` holds elements idx = base(tid) .. ; generic
-// helper used only at flush time (once per task segment), so simplicity beats speed here.
 template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A) {
     using L = PLayout<DO, DA, HID>;
@@ -203,20 +52,22 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
     using R = RoleCfg<HID>;
     using SM = GradSmem<DO, DA, HID>;
     constexpr int LD = C::LD, RM = C::RM, RK = C::RK, DOP = SM::DOP;
-    constexpr int NPART = R::NPART, BPP = R::BPP, QW = R::QW;
+    constexpr int BPP = R::BPP, QW = R::QW;
     constexpr int PSTRIDE = L::P + PSTAT;
+    constexpr int SCR = (int)((offsetof(SM, red) - offsetof(SM, X)) / sizeof(float));    // flush scratch: X .. DLS
 
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SM& S = *reinterpret_cast<SM*>(smem_raw);
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int tx = tid % C::TX, ty = tid / C::TX;
     const int row0 = ty * RM, col0 = tx * 4;
     const int rb = tid >> 2, rq = tid & 3;           // row role
     const int cj = tid % HID, cp = tid / HID;        // column role
     const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);
-    if (grad_reuse_prologue<L::P, L::LS, DA>(A)) return;
-    const TileSched ts(A.M, A.N, A.q);
+    if (reuse_hit<L::P>(A.skip_flag, A.params, A.skip_theta)) return;
+    reuse_produce<L::P, L::LS, DA>(A);
+    const UniformSched sc(A.M, A.N, A.q, A.kmax, TB);
     const int N = A.N;
     const float kl_eff = kl_coeff_eff(A);
     float invN = 1.0f / (float)N;       // both re-set per task when A.n_valid is given (variable-length paths)
@@ -254,12 +105,12 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
             const int j = i / HID, k = i % HID;      // consecutive threads -> consecutive W1T addresses
             S.W1T[j * HID + k] = S.P[L::W1 + k * HID + j];
         }
-        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin, dA);
+        head_setup<DA>(A, S.P + L::LS, m, dA, hin, nullptr);
     };
     // write this CTA's partial sums for task m; the last segment of the task reduces them in CTA order
     auto flush = [&](int m) {
-        float* part = A.partial + ((int64_t)blockIdx.x * A.kmax + (m - ts.first_task(blockIdx.x))) * PSTRIDE;
-        float* scr = S.H1;      // free between tiles
+        float* part = A.partial + (int64_t)sc.my_slot(m) * PSTRIDE;
+        float* scr = S.X;       // X .. DLS: free between tiles (H1 alone is too small for the W0 slices of <20, 2, 32>)
         __syncthreads();
         if (want_grad) {
 #pragma unroll
@@ -285,69 +136,15 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
                 part[L::B0 + tid] = s;
             }
             __syncthreads();
-            // W0 / W2 gradients: reduce the NPART sample slices
-#pragma unroll
-            for (int i = 0; i < DO; ++i) scr[(cp * DO + i) * HID + cj] = gW0p[i];
-            __syncthreads();
-            for (int idx = tid; idx < DO * HID; idx += PT_THREADS) {
-                float s = 0.f;
-                for (int p = 0; p < NPART; ++p) s += scr[p * DO * HID + idx];
-                part[L::W0 + idx] = s;
-            }
-            __syncthreads();
-#pragma unroll
-            for (int d = 0; d < DA; ++d) scr[(cp * HID + cj) * DA + d] = gW2p[d];
-            __syncthreads();
-            for (int idx = tid; idx < HID * DA; idx += PT_THREADS) {
-                float s = 0.f;
-                for (int p = 0; p < NPART; ++p) s += scr[p * HID * DA + idx];
-                part[L::W2 + idx] = s;
-            }
             if (tid < DA) part[L::B2 + tid] = gB2, part[L::LS + tid] = gLS;
         }
-        // head statistics (held by the rq == 0 threads)
-        const float v0 = warp_sum(rq == 0 ? s_obj : 0.f), v1 = warp_sum(rq == 0 ? s_kl : 0.f),
-                    v2 = warp_sum(rq == 0 ? s_ratio : 0.f);
-        __syncthreads();
-        if (lane == 0) S.red[warp] = v0, S.red[8 + warp] = v1, S.red[16 + warp] = v2;
-        __syncthreads();
-        if (tid < 3) {
-            float s = 0.f;
-            for (int w = 0; w < PT_THREADS / 32; ++w) s += S.red[tid * 8 + w];
-            part[L::P + tid] = s;
-        }
-        __threadfence();
-        __syncthreads();
-        const int c_lo = ts.cta_lo(m), c_hi = ts.cta_hi(m);
-        if (tid == 0) S.last = (atomicAdd(A.counters + m, 1) == c_hi - c_lo);
-        __syncthreads();
-        if (S.last) {
-            __threadfence();
-            if (want_grad) {
-                static_assert(L::P % 4 == 0 && PSTRIDE % 4 == 0, "float4 reduction needs P % 4 == 0");
-                for (int p = 4 * tid; p < L::P; p += 4 * PT_THREADS) {
-                    const float4 s = reduce_segments4(A.partial, ts, A.kmax, PSTRIDE, m, c_lo, c_hi, p);
-                    *reinterpret_cast<float4*>(A.grad + (int64_t)m * L::P + p) = s;
-                    if (A.out_params)      // meta_algos/base.py:209
-                        *reinterpret_cast<float4*>(A.out_params + (int64_t)m * L::P + p) =
-                            make_float4(S.P[p] - A.sgd_lr * s.x, S.P[p + 1] - A.sgd_lr * s.y, S.P[p + 2] - A.sgd_lr * s.z,
-                                        S.P[p + 3] - A.sgd_lr * s.w);
-                }
-            }
-            if (A.stats && tid < 3) {
-                float s = 0.f;
-                for (int c = c_lo; c <= c_hi; ++c)
-                    s += __ldcg(A.partial + ((int64_t)c * A.kmax + (m - ts.first_task(c))) * PSTRIDE + L::P + tid);
-                A.stats[(int64_t)m * 4 + tid] = s * invN;
-            }
-            if (tid == 0) A.counters[m] = 0;
-        }
-        __syncthreads();
+        flush_tail<PT_THREADS, 2, SCR, DO, DA, HID>(A, sc, m, invN, want_grad, part, scr, S.red, S.last, gW0p, gW2p, s_obj, s_kl, s_ratio,
+                                               GradEpilogue<L::P, UniformSched>{A, th, m});
     };
 
     int cur_m = -1;
-    for (int g = ts.g_lo; g < ts.g_hi; ++g) {
-        const int m = g / ts.ntiles, tile = g - m * ts.ntiles;
+    for (int g = sc.g_lo; g < sc.g_hi; ++g) {
+        const int m = g / sc.ntiles, tile = g - m * sc.ntiles;
         if (m != cur_m) {
             if (cur_m >= 0) flush(cur_m);
             load_task(m, cur_m < 0);
@@ -389,7 +186,6 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
         }
         __syncthreads();
         // ---- layer 2 + Gaussian head: 4 threads per sample row, quarter dot products + 2 shuffles
-#ifndef PROMP_EXP_NO_HEAD
         {
             float mu[DA];
 #pragma unroll
@@ -415,25 +211,13 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
             if (rq == 0) {
                 float dmu[DA], dls[DA];
                 if (rb < nb) {
-                    const int64_t n = g0 + rb;
                     float a[DA], mo[DA], lso[DA];
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) {
-                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                        lso[d] = d >= dA ? 0.f : A.ls_per_sample ? __ldg(A.old_ls + n * dA + d) : __ldg(A.old_ls + (int64_t)m * dA + d);
-                    }
-                    const float adv = __ldg(A.adv + n);
+                    const float adv = load_head_sample<DA>(A, g0 + rb, m, dA, true, a, mo, lso);
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
-                    const float wt = A.obj_scale * o.w * invN, kc = kl_eff * invN;
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) {
-                        dmu[d] = wt * o.zeta[d] * hin.inv_sig[d] + kc * o.dkl_dmu[d];
-                        dls[d] = (wt * (o.zeta[d] * o.zeta[d] - 1.f) + kc * o.dkl_dls[d]) * hin.ls_mask[d];
-                    }
+                    grad_signal<DA>(hin, o, A.obj_scale, kl_eff, invN, dmu, dls);
                     s_obj += o.obj;
                     s_kl += o.kl;
                     s_ratio += o.ratio;
@@ -445,7 +229,6 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
                 for (int d = 0; d < DA; ++d) S.DMU[rb * DA + d] = dmu[d], S.DLS[rb * DA + d] = dls[d];
             }
         }
-#endif
         if (!want_grad) continue;
         __syncthreads();
         // ---- output layer gradients (column role): gW2[cj][d] += sum_{b in slice} H2[b][cj] * DMU[b][d]
@@ -549,25 +332,27 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
     using R = RoleCfg<HID>;
     using SM = HvpSmem<DO, DA, HID>;
     constexpr int LD = C::LD, RM = C::RM, RK = C::RK, DOP = SM::DOP;
-    constexpr int NPART = R::NPART, BPP = R::BPP, QW = R::QW;
+    constexpr int BPP = R::BPP, QW = R::QW;
     constexpr int PSTRIDE = L::P + PSTAT;
+    constexpr int SCR = (int)((offsetof(SM, red) - offsetof(SM, H1)) / sizeof(float));   // flush scratch: H1 .. CLS
 
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SM& S = *reinterpret_cast<SM*>(smem_raw);
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tid = threadIdx.x;
     const int tx = tid % C::TX, ty = tid / C::TX;
     const int row0 = ty * RM, col0 = tx * 4;
     const int rb = tid >> 2, rq = tid & 3;
     const int cj = tid % HID, cp = tid / HID;
     const int dO = obs_dim_of<DO, DA>(A), dA = act_dim_of<DO, DA>(A);
-    const TileSched ts(A.M, A.N, A.q);
+    const UniformSched sc(A.M, A.N, A.q, A.kmax, TB);
     const int N = A.N;
     const float kl_eff = kl_coeff_eff(A);
     float invN = 1.0f / (float)N;       // both re-set per task when A.n_valid is given (variable-length paths)
     int Nm = N;
     const float ac = -A.inner_lr;                 // coefficient of H vec in `out`
     const float* th = nullptr;
+    const float* vg = nullptr;
     HeadIn<DA> hin;
     float rls[DA];     // tangent of the (clipped) log_std
 
@@ -592,7 +377,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
     auto load_task = [&](int m, bool first) {
         if (A.n_valid) { Nm = __ldg(A.n_valid + m); invN = 1.0f / (float)max(Nm, 1); }
         th = A.params + (int64_t)m * A.param_stride;
-        const float* vg = A.vec + (int64_t)m * L::P;
+        vg = A.vec + (int64_t)m * L::P;
         const bool reload_p = first || A.param_stride != 0;      // shared theta stays resident across tasks
         __syncthreads();
         for (int i = tid; i < L::P; i += PT_THREADS) {
@@ -605,13 +390,13 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             if (reload_p) S.W1T[j * HID + k] = S.P[L::W1 + k * HID + j];
             S.V1T[j * HID + k] = S.V[L::W1 + k * HID + j];
         }
-        load_head_consts<DO, DA, HID>(S.P, A.clip_log_std, A.min_log_std, hin, dA);
+        head_setup<DA>(A, S.P + L::LS, m, dA, hin, nullptr);
 #pragma unroll
         for (int d = 0; d < DA; ++d) rls[d] = S.V[L::LS + d] * hin.ls_mask[d];
     };
     auto flush = [&](int m) {
-        float* part = A.partial + ((int64_t)blockIdx.x * A.kmax + (m - ts.first_task(blockIdx.x))) * PSTRIDE;
-        float* scr = S.H1;
+        float* part = A.partial + (int64_t)sc.my_slot(m) * PSTRIDE;
+        float* scr = S.H1;      // H1 .. CLS: free between tiles
         __syncthreads();
 #pragma unroll
         for (int r = 0; r < RK; ++r)
@@ -635,61 +420,14 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             part[L::B0 + tid] = s;
         }
         __syncthreads();
-#pragma unroll
-        for (int i = 0; i < DO; ++i) scr[(cp * DO + i) * HID + cj] = gW0p[i];
-        __syncthreads();
-        for (int idx = tid; idx < DO * HID; idx += PT_THREADS) {
-            float s = 0.f;
-            for (int p = 0; p < NPART; ++p) s += scr[p * DO * HID + idx];
-            part[L::W0 + idx] = s;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int d = 0; d < DA; ++d) scr[(cp * HID + cj) * DA + d] = gW2p[d];
-        __syncthreads();
-        for (int idx = tid; idx < HID * DA; idx += PT_THREADS) {
-            float s = 0.f;
-            for (int p = 0; p < NPART; ++p) s += scr[p * HID * DA + idx];
-            part[L::W2 + idx] = s;
-        }
         if (tid < DA) part[L::B2 + tid] = gB2, part[L::LS + tid] = gLS;
-        const float v0 = warp_sum(rq == 0 ? s_obj : 0.f), v1 = warp_sum(rq == 0 ? s_kl : 0.f),
-                    v2 = warp_sum(rq == 0 ? s_ratio : 0.f);
-        __syncthreads();
-        if (lane == 0) S.red[warp] = v0, S.red[8 + warp] = v1, S.red[16 + warp] = v2;
-        __syncthreads();
-        if (tid < 3) {
-            float s = 0.f;
-            for (int w = 0; w < PT_THREADS / 32; ++w) s += S.red[tid * 8 + w];
-            part[L::P + tid] = s;
-        }
-        __threadfence();
-        __syncthreads();
-        const int c_lo = ts.cta_lo(m), c_hi = ts.cta_hi(m);
-        if (tid == 0) S.last = (atomicAdd(A.counters + m, 1) == c_hi - c_lo);
-        __syncthreads();
-        if (S.last) {
-            __threadfence();
-            static_assert(L::P % 4 == 0 && PSTRIDE % 4 == 0, "float4 reduction needs P % 4 == 0");
-            for (int p = 4 * tid; p < L::P; p += 4 * PT_THREADS) {
-                const float4 s = reduce_segments4(A.partial, ts, A.kmax, PSTRIDE, m, c_lo, c_hi, p);
-                *reinterpret_cast<float4*>(A.out + (int64_t)m * L::P + p) =
-                    make_float4(S.V[p] + s.x, S.V[p + 1] + s.y, S.V[p + 2] + s.z, S.V[p + 3] + s.w);
-            }
-            if (A.stats && tid < 3) {
-                float s = 0.f;
-                for (int c = c_lo; c <= c_hi; ++c)
-                    s += __ldcg(A.partial + ((int64_t)c * A.kmax + (m - ts.first_task(c))) * PSTRIDE + L::P + tid);
-                A.stats[(int64_t)m * 4 + tid] = s * invN;
-            }
-            if (tid == 0) A.counters[m] = 0;
-        }
-        __syncthreads();
+        flush_tail<PT_THREADS, 2, SCR, DO, DA, HID>(A, sc, m, invN, true, part, scr, S.red, S.last, gW0p, gW2p, s_obj, s_kl, s_ratio,
+                                               HvpEpilogue<L::P>{A, vg, m});
     };
 
     int cur_m = -1;
-    for (int g = ts.g_lo; g < ts.g_hi; ++g) {
-        const int m = g / ts.ntiles, tile = g - m * ts.ntiles;
+    for (int g = sc.g_lo; g < sc.g_hi; ++g) {
+        const int m = g / sc.ntiles, tile = g - m * sc.ntiles;
         if (m != cur_m) {
             if (cur_m >= 0) flush(cur_m);
             load_task(m, cur_m < 0);
@@ -754,7 +492,6 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
         }
         __syncthreads();
         // ---- layer 2, its tangent, and the Gaussian head with its tangent (row role)
-#ifndef PROMP_EXP_NO_HEAD
         {
             float mu[DA], rmu[DA];
 #pragma unroll
@@ -786,38 +523,13 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             if (rq == 0) {
                 float dmu[DA], cmu[DA], cls[DA];
                 if (rb < nb) {
-                    const int64_t n = g0 + rb;
                     float a[DA], mo[DA], lso[DA];
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) {
-                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                        lso[d] = d >= dA ? 0.f : A.ls_per_sample ? __ldg(A.old_ls + n * dA + d) : __ldg(A.old_ls + (int64_t)m * dA + d);
-                    }
-                    const float adv = __ldg(A.adv + n);
+                    const float adv = load_head_sample<DA>(A, g0 + rb, m, dA, true, a, mo, lso);
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
-                    const float wt = o.w * invN, kc = kl_eff * invN;
-                    // tangent of log p:  R l = sum_d (zeta/sig) R mu + (zeta^2 - 1) R ls
-                    float rl = 0.f;
-#pragma unroll
-                    for (int d = 0; d < DA; ++d)
-                        rl += (o.zeta[d] * hin.inv_sig[d]) * rmu[d] + (o.zeta[d] * o.zeta[d] - 1.f) * rls[d];
-                    // d w / d logp: RATIO w = -A r -> R w = w R l ; LOGLIK w = -A -> 0
-                    const float rwt = (A.obj_kind == PROMP_OBJ_RATIO) ? wt * rl : 0.f;
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) {
-                        const float is = hin.inv_sig[d], z = o.zeta[d];
-                        const float rz = -rmu[d] * is - z * rls[d];
-                        dmu[d] = wt * z * is;
-                        const float rdmu = rwt * z * is + wt * (rz * is - z * rls[d] * is);
-                        const float rdls = rwt * (z * z - 1.f) + wt * 2.f * z * rz;
-                        cmu[d] = ac * rdmu + kc * o.dkl_dmu[d];
-                        cls[d] = (ac * rdls + kc * o.dkl_dls[d]) * hin.ls_mask[d];
-                        if (d >= dA) dmu[d] = cmu[d] = 0.f;      // padding: exactly zero whatever the direction's pad entries hold
-                    }
+                    hvp_signal<DA>(hin, o, rmu, rls, A.obj_kind, kl_eff, invN, ac, dA, dmu, cmu, cls);
                     s_obj += o.obj;
                     s_kl += o.kl;
                     s_ratio += o.ratio;
@@ -830,7 +542,6 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
                     S.DMU[rb * DA + d] = dmu[d], S.CMU[rb * DA + d] = cmu[d], S.CLS[rb * DA + d] = cls[d];
             }
         }
-#endif
         __syncthreads();
         // ---- output layer (column role): out_W2 += H2^T CMU + ac * R2^T DMU ; out_b2 += colsum CMU ; out_ls += colsum CLS
         {
@@ -924,17 +635,15 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
     if (cur_m >= 0) flush(cur_m);
 }
 
-}  // namespace promp
-#include "policy_tc.cuh"
-namespace promp {
-
 // -------------------------------------------------------------------------------------------------
-// forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling).  dO / dA: the logical sizes
-// (= DO / DA for the exact instantiations, run-time values in policy_forward_padded_kernel)
+// forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling).  obs_dim / act_dim: the
+// logical sizes, read only by the padded instantiations (IsBucket)
 template <int DO, int DA, int HID>
-__device__ __forceinline__ void policy_forward_body(int M, int N, const float* params, int64_t stride, const float* obs,
-                                                    float* mean, int dO, int dA) {
+__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride, const float* obs,
+                                                              float* mean, int obs_dim, int act_dim) {
     using L = PLayout<DO, DA, HID>;
+    constexpr bool BUCKET = IsBucket<DO, DA>::value;
+    const int dO = BUCKET ? obs_dim : DO, dA = BUCKET ? act_dim : DA;
     constexpr int NU = HID / 32;
     __shared__ float sP[L::P];
     __shared__ float sh[4][HID];
@@ -971,16 +680,6 @@ __device__ __forceinline__ void policy_forward_body(int M, int N, const float* p
         }
         __syncwarp();
     }
-}
-template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride,
-                                                              const float* obs, float* mean) {
-    policy_forward_body<DO, DA, HID>(M, N, params, stride, obs, mean, DO, DA);
-}
-template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(128) policy_forward_padded_kernel(int M, int N, const float* params, int64_t stride,
-                                                                     const float* obs, float* mean, int obs_dim, int act_dim) {
-    policy_forward_body<DO, DA, HID>(M, N, params, stride, obs, mean, obs_dim, act_dim);
 }
 
 __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, float* out) {
@@ -1388,13 +1087,8 @@ static int launch_forward(int M, int N, const float* params, int64_t stride, con
     const int cap = (4 * sm_count() + M - 1) / M;
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    if constexpr (IsBucket<DO, DA>::value) {
-        policy_forward_padded_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
-        PROMP_LAUNCH_CHECK("policy_forward_padded_kernel");
-    } else {
-        policy_forward_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean);
-        PROMP_LAUNCH_CHECK("policy_forward_kernel");
-    }
+    policy_forward_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+    PROMP_LAUNCH_CHECK("policy_forward_kernel");
     return PROMP_OK;
 }
 

@@ -234,14 +234,6 @@ __device__ __forceinline__ void load_row(const unsigned char* tile, int r, int c
 }
 
 // -------------------------------------------------------------------------------------------------------------
-// Work decomposition seen by the tile loops below.  Both tensor-core kernels are written against this interface:
-//   [g_lo, g_hi)            the caller's range in the task-major tile list (ntiles tiles per task)
-//   my_slot(m)              partial slot this range writes for task m
-//   n_contrib / contrib_slot the slots of task m, in the fixed order in which its last arriver sums them
-//   wait_task / publish_task dependency on / completion of task m (dataflow kernel only)
-//   ldp                     parameter loads: read-only path (.nc) when nothing in this launch writes them, L2 (.cg) otherwise
-// UniformSched = the stand-alone launches (CTA c owns tiles [c q, (c+1) q), kmax slots per CTA); ItemSched = one work
-// item of policy_chain_tc_kernel (tiles [tile_lo, tile_hi) of ONE task; slots are numbered by item id).
 #ifdef PROMP_EXP_CLOCKS
 // experiment build only: clock64 totals over ALL CTAs of policy_chain_tc_kernel (thread 0 of each CTA):
 // 0 queue pop + decode, 1 dependency wait, 2 parameter / weight load, 3 tiles, 4 flush up to the ticket, 5 last-arriver
@@ -264,30 +256,8 @@ __device__ long long g_chain_last[1024];
 #define CCLK(i)
 #define CCNT(i)
 #endif
-struct UniformSched {
-    int ntiles, g_lo, g_hi, q, kmax;
-    __device__ __forceinline__ UniformSched(int M, int N, int q_, int kmax_, int tb) {
-        ntiles = (N + tb - 1) / tb;
-        q = q_;
-        kmax = kmax_;
-        g_lo = blockIdx.x * q;
-        g_hi = min(g_lo + q, M * ntiles);
-    }
-    __device__ __forceinline__ int first_task(int c) const { return (c * q) / ntiles; }
-    __device__ __forceinline__ int cta_lo(int m) const { return (m * ntiles) / q; }
-    __device__ __forceinline__ int cta_hi(int m) const { return ((m + 1) * ntiles - 1) / q; }
-    __device__ __forceinline__ int my_slot(int m) const { return blockIdx.x * kmax + (m - first_task(blockIdx.x)); }
-    __device__ __forceinline__ int n_contrib(int m) const { return cta_hi(m) - cta_lo(m) + 1; }
-    __device__ __forceinline__ int contrib_slot(int m, int i) const {
-        const int c = cta_lo(m) + i;
-        return c * kmax + (m - first_task(c));
-    }
-    __device__ __forceinline__ void wait_task(int) const {}
-    __device__ __forceinline__ void publish_task(int) const {}
-    __device__ __forceinline__ void clk(int) const {}
-    static __device__ __forceinline__ float ldp(const float* p) { return __ldg(p); }
-    static __device__ __forceinline__ float4 ldp4(const float4* p) { return __ldg(p); }
-};
+// ItemSched: the schedule (see UniformSched in mlp_tile.cuh) of one work item of policy_chain_tc_kernel: tiles
+// [g_lo, g_hi) of ONE task; slots are numbered by item id.
 struct ItemSched {
     int ntiles, g_lo, g_hi;
     int item, first_item, n_items;        // this item's id; the ids of its task's items in this stage
@@ -327,48 +297,6 @@ struct ItemSched {
     static __device__ __forceinline__ float ldp(const float* p) { return __ldcg(p); }
     static __device__ __forceinline__ float4 ldp4(const float4* p) { return __ldcg(p); }
 };
-
-// Sum one float4 column of a task's partial slots in contributor order, eight independent L2 loads in flight.
-template <class Sched>
-__device__ __forceinline__ float4 reduce_slots4(const float* partial, const Sched& sc, int pstride, int m, int n, int p) {
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int i0 = 0; i0 < n; i0 += 8) {
-        float4 v[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u)
-            v[u] = (i0 + u < n) ? __ldcg(reinterpret_cast<const float4*>(partial + (int64_t)sc.contrib_slot(m, i0 + u) * pstride + p))
-                                : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int u = 0; u < 8; ++u) s.x += v[u].x, s.y += v[u].y, s.z += v[u].z, s.w += v[u].w;
-    }
-    return s;
-}
-
-// The same sums for ALL of a thread's columns p = 4 tid + i * 4 * threads (i < NP) at once: NP x 4 independent 16-byte L2 loads
-// in flight instead of one column at a time - the last arriver's reduction sits on the tail of the kernel and is pure L2
-// latency.  Slots are added in contributor order, so the result is bit-identical to reduce_slots4.
-template <int NP, class Sched>
-__device__ __forceinline__ void reduce_slots4_wide(const float* partial, const Sched& sc, int pstride, int m, int n, int p0, int pstep,
-                                                   int pend, float4 (&acc)[NP]) {
-#pragma unroll
-    for (int i = 0; i < NP; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int c0 = 0; c0 < n; c0 += 4) {
-        float4 v[NP][4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int64_t base = (c0 + u < n) ? (int64_t)sc.contrib_slot(m, c0 + u) * pstride : -1;
-#pragma unroll
-            for (int i = 0; i < NP; ++i) {
-                const int p = p0 + i * pstep;
-                v[i][u] = (base >= 0 && p < pend) ? __ldcg(reinterpret_cast<const float4*>(partial + base + p)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u)
-#pragma unroll
-            for (int i = 0; i < NP; ++i) acc[i].x += v[i][u].x, acc[i].y += v[i][u].y, acc[i].z += v[i][u].z, acc[i].w += v[i][u].w;
-    }
-}
 
 #ifdef PROMP_EXP_CLOCKS
 // experiment build only: per-phase clock64 totals of CTA 0 (tools/kernel_time.py --clocks)
@@ -468,30 +396,13 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         }
         if (reload) wg_fence_weights();      // the weight tiles are read by the wgmma (async) proxy after the barrier
         __syncthreads();          // Ps is in place; every reader of the previous task's hin / hold is done
-        if (tid == 0) {
-#pragma unroll
-            for (int d = 0; d < DA; ++d) {
-                const float raw = S.Ps[SL::LS + d];
-                const bool clipped = A.clip_log_std && (raw < A.min_log_std);
-                hin.ls[d] = clipped ? A.min_log_std : raw;
-                hin.ls_mask[d] = (clipped || d >= dA) ? 0.f : 1.f;
-                hin.sig[d] = expf(hin.ls[d]);
-            }
-            head_in_finish<DA>(hin, dA);
-            if (!A.ls_per_sample) {
-                float lso[DA];
-#pragma unroll
-                for (int d = 0; d < DA; ++d) lso[d] = d < dA ? __ldg(A.old_ls + (int64_t)m * dA + d) : 0.f;
-                head_old_from<DA>(lso, S.hold, dA);
-            }
-        }
+        if (tid == 0) head_setup<DA>(A, S.Ps + SL::LS, m, dA, hin, &S.hold);
         __syncthreads();
     };
     auto flush = [&](int m) {
         sc.clk(3);
         float* part = A.partial + (int64_t)sc.my_slot(m) * PSTRIDE;
         float* scr = reinterpret_cast<float*>(S.A1);      // A1 + LO (contiguous, 2 tiles): free between tiles (all MMAs have completed)
-        static_assert(NPART * DO * HID * 4 <= 2 * TILE_A_BYTES && NPART * HID * DA * 4 <= 2 * TILE_A_BYTES, "flush scratch");
         __syncthreads();
         if (want_grad) {
 #pragma unroll
@@ -514,89 +425,18 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
             }
             __syncthreads();
 #pragma unroll
-            for (int i = 0; i < DO; ++i) scr[(cp * DO + i) * HID + cj] = gW0p[i];
-            __syncthreads();
-            for (int idx = tid; idx < DO * HID; idx += TCT) {
-                float s = 0.f;
-                for (int p = 0; p < NPART; ++p) s += scr[p * DO * HID + idx];
-                part[L::W0 + idx] = s;
-            }
-            __syncthreads();
-#pragma unroll
-            for (int d = 0; d < DA; ++d) scr[(cp * HID + cj) * DA + d] = gW2p[d];
-            __syncthreads();
-            for (int idx = tid; idx < HID * DA; idx += TCT) {
-                float s = 0.f;
-                for (int p = 0; p < NPART; ++p) s += scr[p * HID * DA + idx];
-                part[L::W2 + idx] = s;
-            }
-            __syncthreads();
-#pragma unroll
             for (int d = 0; d < DA; ++d) {                 // (uniform over the CTA: every warp takes part in the shuffles)
                 const float s1 = warp_sum(gB2w[d]), s2 = warp_sum(gLSw[d]);
                 if (cq == 0 && lane == 0) scr[qd * 2 * DA + d] = s1, scr[qd * 2 * DA + DA + d] = s2;
             }
             __syncthreads();
             if (tid < 2 * DA) part[L::B2 + tid] = scr[tid] + scr[2 * DA + tid] + scr[4 * DA + tid] + scr[6 * DA + tid];   // b2 then log_std
+            __syncthreads();
         }
-        const float v0 = warp_sum(s_obj), v1 = warp_sum(s_kl), v2 = warp_sum(s_ratio);   // held by cq == 0 threads, 0 elsewhere
-        __syncthreads();
-        if (lane == 0) S.red[warp] = v0, S.red[NW + warp] = v1, S.red[2 * NW + warp] = v2;
-        __syncthreads();
-        if (tid < 3) {
-            float s = 0.f;
-            for (int w = 0; w < NW; ++w) s += S.red[tid * NW + w];
-            part[L::P + tid] = s;
-        }
-        __syncthreads();
         PCLK(14);
-        const int n_c = sc.n_contrib(m);
-        if (tid == 0) {          // release by ONE thread: the barrier above orders the CTA's partial-slot writes before this fence
-            __threadfence();
-            S.last = (atomicAdd(A.counters + m, 1) == n_c - 1);
-        }
-        __syncthreads();
+        flush_tail<TCT, 8, 2 * TILE_A_BYTES / 4, DO, DA, HID>(A, sc, m, invN, want_grad, part, scr, S.red, S.last, gW0p, gW2p, s_obj, s_kl, s_ratio,
+                                        GradEpilogue<L::P, Sched>{A, th, m});
         PCLK(15);
-        sc.clk(4);
-        if (S.last) {
-            __threadfence();
-            // the trailing float4 of every partial slot holds the objective / KL / ratio sums: reduced by the same loop
-            static_assert(L::P % 4 == 0 && PSTAT == 4, "stats ride on the float4 reduction");
-            if (!want_grad && tid == 0 && A.stats) {
-                const float4 s = reduce_slots4(A.partial, sc, PSTRIDE, m, n_c, L::P);
-                A.stats[(int64_t)m * 4 + 0] = s.x * invN, A.stats[(int64_t)m * 4 + 1] = s.y * invN, A.stats[(int64_t)m * 4 + 2] = s.z * invN;
-            }
-            if (want_grad) {
-                constexpr int NPASS = (L::P + 4 + 4 * TCT - 1) / (4 * TCT);
-                float4 sum[NPASS], t4[NPASS];
-#pragma unroll
-                for (int i = 0; i < NPASS; ++i) {          // requested together with the slot loads below
-                    const int p = 4 * tid + i * 4 * TCT;
-                    t4[i] = (A.out_params && p < L::P) ? Sched::ldp4(reinterpret_cast<const float4*>(th + p)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-                reduce_slots4_wide<NPASS>(A.partial, sc, PSTRIDE, m, n_c, 4 * tid, 4 * TCT, L::P + 4, sum);
-#pragma unroll
-                for (int i = 0; i < NPASS; ++i) {
-                    const int p = 4 * tid + i * 4 * TCT;
-                    const float4 s = sum[i];
-                    if (p == L::P) {
-                        if (A.stats)
-                            A.stats[(int64_t)m * 4 + 0] = s.x * invN, A.stats[(int64_t)m * 4 + 1] = s.y * invN,
-                                                    A.stats[(int64_t)m * 4 + 2] = s.z * invN;
-                    } else if (p < L::P) {
-                        *reinterpret_cast<float4*>(A.grad + (int64_t)m * L::P + p) = s;
-                        if (A.out_params)
-                            *reinterpret_cast<float4*>(A.out_params + (int64_t)m * L::P + p) =
-                                make_float4(t4[i].x - A.sgd_lr * s.x, t4[i].y - A.sgd_lr * s.y, t4[i].z - A.sgd_lr * s.z,
-                                            t4[i].w - A.sgd_lr * s.w);
-                    }
-                }
-            }
-            if (tid == 0) A.counters[m] = 0;
-            sc.publish_task(m);
-            sc.clk(5);
-        }
-        __syncthreads();
     };
 
     // observation prefetch (small observation / action spaces: one or two elements per thread, registers to spare)
@@ -635,16 +475,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #pragma unroll
             for (int e = 0; e < XR; ++e) S.X[tid + e * TCT] = xq[e];
             if (g + 1 < sc.g_hi) fetch_x(g + 1, xq);
-            if (cq == 0 && r < nb) {
-                const int64_t n = g0 + r;
-#pragma unroll
-                for (int d = 0; d < DA; ++d) {
-                    ha[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                    hmo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                    if (A.ls_per_sample) hlso[d] = d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
-                }
-                hadv = __ldg(A.adv + n);
-            }
+            if (cq == 0 && r < nb) hadv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, ha, hmo, hlso);
         } else {
             for (int i = tid; i < TBT * DOP; i += TCT) {
                 const int b = i / DOP, c = i % DOP;
@@ -710,39 +541,31 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         if (cq == 0) {
             float dmu[DA], dls[DA];
             if (r < nb) {
-                const int64_t n = g0 + r;
-                float mu[DA], a[DA], mo[DA];
+                float mu[DA];
 #pragma unroll
                 for (int d = 0; d < DA; ++d) {
                     float sm = S.Ps[SL::B2 + d];
 #pragma unroll
                     for (int q = 0; q < NQ; ++q) sm += S.MUP[(q * TBT + r) * DA + d];
                     mu[d] = sm;
-                    if constexpr (XPRE) {
-                        a[d] = ha[d], mo[d] = hmo[d];
-                    } else {
-                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                    }
                 }
-                const float adv = XPRE ? hadv : __ldg(A.adv + n);
+                float a[DA], mo[DA], lso[DA], adv;
+                if constexpr (XPRE) {
+#pragma unroll
+                    for (int d = 0; d < DA; ++d) a[d] = ha[d], mo[d] = hmo[d], lso[d] = hlso[d];
+                    adv = hadv;
+                } else {
+                    adv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
+                }
                 HeadOut<DA> o;
                 if (A.ls_per_sample) {
-                    float lso[DA];
                     HeadOld<DA> ho;
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
                     head_old_from<DA>(lso, ho, dA);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 } else {
                     gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
-                const float wt = A.obj_scale * o.w * invN, kc = kl_eff * invN;
-#pragma unroll
-                for (int d = 0; d < DA; ++d) {
-                    dmu[d] = wt * o.zeta[d] * hin.inv_sig[d] + kc * o.dkl_dmu[d];
-                    dls[d] = (wt * (o.zeta[d] * o.zeta[d] - 1.f) + kc * o.dkl_dls[d]) * hin.ls_mask[d];
-                }
+                grad_signal<DA>(hin, o, A.obj_scale, kl_eff, invN, dmu, dls);
                 s_obj += o.obj;
                 s_kl += o.kl;
                 s_ratio += o.ratio;
@@ -853,7 +676,8 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs 
     using L = PLayout<DO, DA, TC_HID>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SM& S = *reinterpret_cast<SM*>(smem_raw);
-    if (grad_reuse_prologue<L::P, L::LS, DA>(A)) return;
+    if (reuse_hit<L::P>(A.skip_flag, A.params, A.skip_theta)) return;
+    reuse_produce<L::P, L::LS, DA>(A);
     const UniformSched sc(A.M, A.N, A.q, A.kmax, TBT);
     const float* cached_th = nullptr;
     grad_tc_tiles<DO, DA, NQ>(A, S, sc, cached_th);
@@ -963,23 +787,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
             S.Vs[SL::W2 + i] = ldv(vg + L::W2 + i);
         }
         __syncthreads();
-        if (tid == 0) {
-#pragma unroll
-            for (int d = 0; d < DA; ++d) {
-                const float raw = S.Ps[SL::LS + d];
-                const bool clipped = A.clip_log_std && (raw < A.min_log_std);
-                hin.ls[d] = clipped ? A.min_log_std : raw;
-                hin.ls_mask[d] = (clipped || d >= dA) ? 0.f : 1.f;
-                hin.sig[d] = expf(hin.ls[d]);
-            }
-            head_in_finish<DA>(hin, dA);
-            if (!A.ls_per_sample) {
-                float lso[DA];
-#pragma unroll
-                for (int d = 0; d < DA; ++d) lso[d] = d < dA ? __ldg(A.old_ls + (int64_t)m * dA + d) : 0.f;
-                head_old_from<DA>(lso, S.hold, dA);
-            }
-        }
+        if (tid == 0) head_setup<DA>(A, S.Ps + SL::LS, m, dA, hin, &S.hold);
         __syncthreads();
 #pragma unroll
         for (int d = 0; d < DA; ++d) rls[d] = S.Vs[SL::LS + d] * hin.ls_mask[d];
@@ -1018,7 +826,6 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
         sc.clk(3);
         float* part = A.partial + (int64_t)sc.my_slot(m) * PSTRIDE;
         float* scr = reinterpret_cast<float*>(S.T2a);     // T2a + T2b (contiguous, 2 tiles)
-        static_assert(NPART * DO * HID * 4 <= 2 * TILE_A_BYTES && NPART * HID * DA * 4 <= 2 * TILE_A_BYTES, "flush scratch");
         __syncthreads();
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt)
@@ -1040,75 +847,15 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
         }
         __syncthreads();
 #pragma unroll
-        for (int i = 0; i < DO; ++i) scr[(cp * DO + i) * HID + cj] = gW0p[i];
-        __syncthreads();
-        for (int idx = tid; idx < DO * HID; idx += TCT) {
-            float s = 0.f;
-            for (int p = 0; p < NPART; ++p) s += scr[p * DO * HID + idx];
-            part[L::W0 + idx] = s;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int d = 0; d < DA; ++d) scr[(cp * HID + cj) * DA + d] = gW2p[d];
-        __syncthreads();
-        for (int idx = tid; idx < HID * DA; idx += TCT) {
-            float s = 0.f;
-            for (int p = 0; p < NPART; ++p) s += scr[p * HID * DA + idx];
-            part[L::W2 + idx] = s;
-        }
-        __syncthreads();
-#pragma unroll
         for (int d = 0; d < DA; ++d) {                     // (uniform over the CTA: every warp takes part in the shuffles)
             const float s1 = warp_sum(gB2w[d]), s2 = warp_sum(gLSw[d]);
             if (cq == 0 && lane == 0) scr[qd * 2 * DA + d] = s1, scr[qd * 2 * DA + DA + d] = s2;
         }
         __syncthreads();
-        if (tid < 2 * DA) part[L::B2 + tid] = scr[tid] + scr[2 * DA + tid] + scr[4 * DA + tid] + scr[6 * DA + tid];
-        const float v0 = warp_sum(s_obj), v1 = warp_sum(s_kl), v2 = warp_sum(s_ratio);
+        if (tid < 2 * DA) part[L::B2 + tid] = scr[tid] + scr[2 * DA + tid] + scr[4 * DA + tid] + scr[6 * DA + tid];   // b2 then log_std
         __syncthreads();
-        if (lane == 0) S.red[warp] = v0, S.red[NW + warp] = v1, S.red[2 * NW + warp] = v2;
-        __syncthreads();
-        if (tid < 3) {
-            float s = 0.f;
-            for (int w = 0; w < NW; ++w) s += S.red[tid * NW + w];
-            part[L::P + tid] = s;
-        }
-        __syncthreads();
-        const int n_c = sc.n_contrib(m);
-        if (tid == 0) {          // release by ONE thread: the barrier above orders the CTA's partial-slot writes before this fence
-            __threadfence();
-            S.last = (atomicAdd(A.counters + m, 1) == n_c - 1);
-        }
-        __syncthreads();
-        sc.clk(4);
-        if (S.last) {
-            __threadfence();
-            constexpr int NPASS = (L::P + 4 + 4 * TCT - 1) / (4 * TCT);
-            float4 sum[NPASS], v4[NPASS];
-#pragma unroll
-            for (int i = 0; i < NPASS; ++i) {              // requested together with the slot loads below
-                const int p = 4 * tid + i * 4 * TCT;
-                v4[i] = (p < L::P) ? __ldcg(reinterpret_cast<const float4*>(vg + p)) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-            reduce_slots4_wide<NPASS>(A.partial, sc, PSTRIDE, m, n_c, 4 * tid, 4 * TCT, L::P + 4, sum);
-#pragma unroll
-            for (int i = 0; i < NPASS; ++i) {
-                const int p = 4 * tid + i * 4 * TCT;
-                const float4 s = sum[i];
-                if (p == L::P) {                  // trailing float4 of the slot: objective / KL / ratio sums
-                    if (A.stats)
-                        A.stats[(int64_t)m * 4 + 0] = s.x * invN, A.stats[(int64_t)m * 4 + 1] = s.y * invN,
-                                                A.stats[(int64_t)m * 4 + 2] = s.z * invN;
-                } else if (p < L::P) {
-                    *reinterpret_cast<float4*>(A.out + (int64_t)m * L::P + p) =
-                        make_float4(v4[i].x + s.x, v4[i].y + s.y, v4[i].z + s.z, v4[i].w + s.w);
-                }
-            }
-            if (tid == 0) A.counters[m] = 0;
-            sc.publish_task(m);
-            sc.clk(5);
-        }
-        __syncthreads();
+        flush_tail<TCT, 8, 2 * TILE_A_BYTES / 4, DO, DA, HID>(A, sc, m, invN, true, part, scr, S.red, S.last, gW0p, gW2p, s_obj, s_kl, s_ratio,
+                                        HvpEpilogue<L::P>{A, vg, m});
     };
 
     constexpr int XR = (TBT * DOP) / TCT;
@@ -1147,16 +894,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
 #pragma unroll
             for (int e = 0; e < XR; ++e) xc[e] = xq[e], sX[tid + e * TCT] = xc[e];
             if (g + 1 < sc.g_hi) fetch_x(g + 1, xq);
-            if (cq == 0 && r < nb) {
-                const int64_t n = g0 + r;
-#pragma unroll
-                for (int d = 0; d < DA; ++d) {
-                    ha[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                    hmo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                    if (A.ls_per_sample) hlso[d] = d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
-                }
-                hadv = __ldg(A.adv + n);
-            }
+            if (cq == 0 && r < nb) hadv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, ha, hmo, hlso);
         } else {
             load_x();
         }
@@ -1240,51 +978,32 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
         if (cq == 0) {
             float dmu[DA], cmu[DA], cls[DA];
             if (r < nb) {
-                const int64_t n = g0 + r;
-                float mu[DA], rmu[DA], a[DA], mo[DA];
+                float mu[DA], rmu[DA];
 #pragma unroll
                 for (int d = 0; d < DA; ++d) {
-float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
+                    float sm = S.Ps[SL::B2 + d], sr = S.Vs[SL::B2 + d];
 #pragma unroll
                     for (int q = 0; q < NQ; ++q) sm += sMUP[((q * TBT + r) * 2 + 0) * DA + d], sr += sMUP[((q * TBT + r) * 2 + 1) * DA + d];
                     mu[d] = sm;
                     rmu[d] = sr;
-                    if constexpr (XPRE) {
-                        a[d] = ha[d], mo[d] = hmo[d];
-                    } else {
-                        a[d] = d < dA ? __ldg(A.act + n * dA + d) : 0.f;
-                        mo[d] = d < dA ? __ldg(A.old_mean + n * dA + d) : 0.f;
-                    }
                 }
-                const float adv = XPRE ? hadv : __ldg(A.adv + n);
+                float a[DA], mo[DA], lso[DA], adv;
+                if constexpr (XPRE) {
+#pragma unroll
+                    for (int d = 0; d < DA; ++d) a[d] = ha[d], mo[d] = hmo[d], lso[d] = hlso[d];
+                    adv = hadv;
+                } else {
+                    adv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
+                }
                 HeadOut<DA> o;
                 if (A.ls_per_sample) {
-                    float lso[DA];
                     HeadOld<DA> ho;
-#pragma unroll
-                    for (int d = 0; d < DA; ++d) lso[d] = XPRE ? hlso[d] : d < dA ? __ldg(A.old_ls + n * dA + d) : 0.f;
                     head_old_from<DA>(lso, ho, dA);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 } else {
                     gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
-                const float wt = o.w * invN, kc = kl_eff * invN;
-                float rl_ = 0.f;
-#pragma unroll
-                for (int d = 0; d < DA; ++d)
-                    rl_ += (o.zeta[d] * hin.inv_sig[d]) * rmu[d] + (o.zeta[d] * o.zeta[d] - 1.f) * rls[d];
-                const float rwt = (A.obj_kind == PROMP_OBJ_RATIO) ? wt * rl_ : 0.f;
-#pragma unroll
-                for (int d = 0; d < DA; ++d) {
-                    const float is = hin.inv_sig[d], z = o.zeta[d];
-                    const float rz = -rmu[d] * is - z * rls[d];
-                    dmu[d] = wt * z * is;
-                    const float rdmu = rwt * z * is + wt * (rz * is - z * rls[d] * is);
-                    const float rdls = rwt * (z * z - 1.f) + wt * 2.f * z * rz;
-                    cmu[d] = ac * rdmu + kc * o.dkl_dmu[d];
-                    cls[d] = (ac * rdls + kc * o.dkl_dls[d]) * hin.ls_mask[d];
-                    if (d >= dA) dmu[d] = cmu[d] = 0.f;      // padding: exactly zero whatever the direction's pad entries hold
-                }
+                hvp_signal<DA>(hin, o, rmu, rls, A.obj_kind, kl_eff, invN, ac, dA, dmu, cmu, cls);
                 s_obj += o.obj;
                 s_kl += o.kl;
                 s_ratio += o.ratio;
@@ -1472,13 +1191,7 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_chain_tc_kernel(const __gr
     const int tid = threadIdx.x;
 
     // launch re-use: stage 0 repeats an earlier stand-alone launch whose outputs are still in place (see promp_policy_grad_ex)
-    bool skip0 = false;
-    if (C.skip_flag) {
-        bool same = *reinterpret_cast<const volatile int*>(C.skip_flag) != 0;
-        for (int i = tid; i < L::P && same; i += blockDim.x)
-            same = __float_as_uint(__ldcg(C.st[0].params + i)) == __float_as_uint(__ldcg(C.skip_theta + i));
-        skip0 = __syncthreads_and(same ? 1 : 0) != 0;
-    }
+    const bool skip0 = reuse_hit<L::P>(C.skip_flag, C.st[0].params, C.skip_theta);
 #ifdef PROMP_EXP_CLOCKS
     if (tid == 0) g_chain_last[blockIdx.x] = clock64();
     const long long t_begin = clock64();
