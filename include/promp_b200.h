@@ -58,6 +58,12 @@ enum {
     PROMP_OBJ_CLIP = 2,    /* -mean(min(r*adv, clip(r,1-e,1+e)*adv)) meta_algos/pro_mp.py:135-141        */
     PROMP_OBJ_NONE = 3     /* only the kl_coeff * mean KL(old||new) term                                 */
 };
+/* Hidden non-linearity of the policy (policies/networks/mlp.py: hidden_nonlinearity), carried in the `hidden` argument of
+ * the policy and rollout entry points: hidden = width | flag, width 32 or 64 in the low byte.  No flag = tanh, so a plain
+ * width keeps its meaning.  ReLU follows TensorFlow's gradient at 0 (sigma'(0) = 0).  Other bits are rejected.
+ * promp_num_params, promp_policy_layout and the workspace sizes do not depend on the activation. */
+#define PROMP_HIDDEN_WIDTH_MASK 0xFF
+#define PROMP_ACT_RELU 0x100
 /* baseline kinds of promp_process_samples */
 enum { PROMP_BASELINE_ZERO = 0, PROMP_BASELINE_LINEAR_FEATURE = 1 };
 

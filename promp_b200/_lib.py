@@ -19,6 +19,8 @@ INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE = 0, 1, 2, 3
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE = 0, 1
+# the policy / rollout `hidden` argument: width | activation flag (no flag = tanh)
+HIDDEN_WIDTH_MASK, ACT_RELU = 0xFF, 0x100
 
 _P = c_void_p
 

@@ -69,6 +69,48 @@ __device__ __forceinline__ float tanh_fast(float x) {
     return fmaf(-2.0f, r, 1.0f);
 }
 
+// ---------------------------------------------------------------- hidden-layer activations
+// Every policy kernel takes its hidden non-linearity as a template parameter.  The kernels keep the activation OUTPUT h,
+// so the derivatives are written in terms of h:
+//   f(z)     = sigma(z)
+//   d(h)     = sigma'(z)
+//   dd_d(h)  = sigma''(z) / sigma'(z).  The Hessian-vector kernels carry the tangent r = sigma'(z) * zdot of h, and their
+//              second-derivative term sigma''(z) * zdot is dd_d(h) * r (tanh: -2 h r).
+// CURVED = false says sigma'' = 0 everywhere the kernels evaluate it (ReLU): the Hessian-vector kernels drop the
+// second-derivative terms at compile time.
+struct ActTanh {
+    static constexpr bool CURVED = true;
+    __device__ __forceinline__ static float f(float z) { return tanh_fast(z); }
+    __device__ __forceinline__ static float d(float h) { return 1.f - h * h; }
+    __device__ __forceinline__ static float dd_d(float h) { return -2.f * h; }
+};
+// sigma'(0) = 0, as TensorFlow's ReluGrad (the gradient flows only where the output is positive)
+struct ActRelu {
+    static constexpr bool CURVED = false;
+    __device__ __forceinline__ static float f(float z) { return fmaxf(z, 0.f); }
+    __device__ __forceinline__ static float d(float h) { return h > 0.f ? 1.f : 0.f; }
+};
+
+// Backward step of the Hessian-vector product through one hidden layer:  c * sigma'(z) + ac * dh * sigma''(z) * zdot,
+// with h = sigma(z) and r = sigma'(z) * zdot.
+template <class Act>
+__device__ __forceinline__ float act_hvp_back(float c, float dh, float h, float r, float ac) {
+    if constexpr (Act::CURVED) return c * Act::d(h) + ac * dh * (Act::dd_d(h) * r);
+    else return c * Act::d(h);
+}
+
+// The `hidden` argument of the policy and rollout entry points: the width (32 or 64) in the low byte, PROMP_ACT_* flags
+// above it.  A plain width selects tanh.
+inline int decode_hidden(const char* who, int hidden, int& width, bool& relu) {
+    PROMP_REQUIRE((hidden & ~(PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU)) == 0,
+                  "%s: unknown flag bits 0x%x in hidden (%d); known: PROMP_ACT_RELU = 0x%x", who,
+                  hidden & ~(PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU), hidden, PROMP_ACT_RELU);
+    width = hidden & PROMP_HIDDEN_WIDTH_MASK;
+    relu = (hidden & PROMP_ACT_RELU) != 0;
+    PROMP_REQUIRE(!relu || width == 32 || width == 64, "%s: ReLU policies are built for hidden 32 or 64 (got %d)", who, width);
+    return PROMP_OK;
+}
+
 // ---------------------------------------------------------------- warp helpers
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

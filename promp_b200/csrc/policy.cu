@@ -10,7 +10,20 @@
 // segment of each task to arrive (atomic ticket) reduces that task's slots in CTA order -> bitwise
 // run-to-run deterministic sums.  These kernels are fp32-FMA bound (AI ~ 10^2..10^3 FLOP/B).
 #include <string.h>
+#include <type_traits>
 #include "policy_tc.cuh"
+
+// This file is compiled twice: as itself (tanh: every kernel, option, entry point) and through policy_relu.cu, which
+// defines PROMP_POLICY_RELU_TU and compiles only the ReLU instantiations of the templated kernels and launchers
+// (namespace promp::relu_tu below).  Separate translation units keep the tanh kernels' code exactly what it was before
+// ReLU existed, and the two halves compile in parallel.
+#ifdef PROMP_POLICY_RELU_TU
+#define PROMP_POLICY_ACT ActRelu
+#define PROMP_ACT_NS relu_tu
+#else
+#define PROMP_POLICY_ACT ActTanh
+#define PROMP_ACT_NS tanh_tu
+#endif
 
 namespace promp {
 
@@ -45,8 +58,8 @@ struct GradSmem {
     int last;
 };
 
-template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A) {
+template <int DO, int DA, int HID, class Act>
+__device__ __forceinline__ void policy_grad_body(const PolicyArgs& A) {
     using L = PLayout<DO, DA, HID>;
     using C = TileCfg<HID>;
     using R = RoleCfg<HID>;
@@ -159,7 +172,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
             S.X[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
         }
         __syncthreads();
-        // ---- layer 0: H1 = tanh(X W0 + b0)                      (policies/networks/mlp.py:96-117)
+        // ---- layer 0: H1 = act(X W0 + b0)                       (policies/networks/mlp.py:96-117)
         {
             float acc[RM][4];
             const float4 bv = *reinterpret_cast<const float4*>(S.P + L::B0 + col0);
@@ -169,10 +182,10 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
 #pragma unroll
             for (int i = 0; i < RM; ++i)
                 *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0) =
-                    make_float4(tanh_fast(acc[i][0]), tanh_fast(acc[i][1]), tanh_fast(acc[i][2]), tanh_fast(acc[i][3]));
+                    make_float4(Act::f(acc[i][0]), Act::f(acc[i][1]), Act::f(acc[i][2]), Act::f(acc[i][3]));
         }
         __syncthreads();
-        // ---- layer 1: H2 = tanh(H1 W1 + b1)
+        // ---- layer 1: H2 = act(H1 W1 + b1)
         {
             float acc[RM][4];
             const float4 bv = *reinterpret_cast<const float4*>(S.P + L::B1 + col0);
@@ -182,7 +195,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
 #pragma unroll
             for (int i = 0; i < RM; ++i)
                 *reinterpret_cast<float4*>(S.H2 + (row0 + i) * LD + col0) =
-                    make_float4(tanh_fast(acc[i][0]), tanh_fast(acc[i][1]), tanh_fast(acc[i][2]), tanh_fast(acc[i][3]));
+                    make_float4(Act::f(acc[i][0]), Act::f(acc[i][1]), Act::f(acc[i][2]), Act::f(acc[i][3]));
         }
         __syncthreads();
         // ---- layer 2 + Gaussian head: 4 threads per sample row, quarter dot products + 2 shuffles
@@ -249,7 +262,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
             }
         }
         __syncthreads();
-        // ---- D2 = (DMU W2^T) * (1 - H2^2), in place over H2; bias gradient accumulates on the fly
+        // ---- D2 = (DMU W2^T) * act'(H2), in place over H2; bias gradient accumulates on the fly
 #pragma unroll
         for (int i = 0; i < RM; ++i) {
             const int b = row0 + i;
@@ -260,7 +273,7 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
                 float dh = 0.f;
 #pragma unroll
                 for (int d = 0; d < DA; ++d) dh = fmaf(S.DMU[b * DA + d], S.P[L::W2 + (col0 + c) * DA + d], dh);
-                o4[c] = dh * (1.f - hv[c] * hv[c]);
+                o4[c] = dh * Act::d(hv[c]);
                 gB1p[c] += o4[c];
             }
             *reinterpret_cast<float4*>(S.H2 + b * LD + col0) = make_float4(o4[0], o4[1], o4[2], o4[3]);
@@ -276,8 +289,8 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
 #pragma unroll
         for (int i = 0; i < RM; ++i) {
             float4 h = *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0);
-            const float4 d1 = make_float4(acc[i][0] * (1.f - h.x * h.x), acc[i][1] * (1.f - h.y * h.y),
-                                          acc[i][2] * (1.f - h.z * h.z), acc[i][3] * (1.f - h.w * h.w));
+            const float4 d1 = make_float4(acc[i][0] * Act::d(h.x), acc[i][1] * Act::d(h.y), acc[i][2] * Act::d(h.z),
+                                          acc[i][3] * Act::d(h.w));
             gB0p[0] += d1.x; gB0p[1] += d1.y; gB0p[2] += d1.z; gB0p[3] += d1.w;
             *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0) = d1;
         }
@@ -296,6 +309,12 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A
     }
     if (cur_m >= 0) flush(cur_m);
 }
+
+// One kernel per activation (the tanh kernels keep their names): *_kernel = tanh, *_relu_kernel = ReLU
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A) { policy_grad_body<DO, DA, HID, ActTanh>(A); }
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_relu_kernel(PolicyArgs A) { policy_grad_body<DO, DA, HID, ActRelu>(A); }
 
 // -------------------------------------------------------------------------------------------------
 // Exact Hessian-vector product of the inner surrogate (R-operator: forward-mode tangent through the
@@ -325,8 +344,8 @@ struct HvpSmem {
     int last;
 };
 
-template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
+template <int DO, int DA, int HID, class Act>
+__device__ __forceinline__ void policy_hvp_body(const PolicyArgs& A) {
     using L = PLayout<DO, DA, HID>;
     using C = TileCfg<HID>;
     using R = RoleCfg<HID>;
@@ -442,7 +461,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             S.X[i] = (b < nb && c < dO) ? __ldg(A.obs + (g0 + b) * dO + c) : 0.f;
         }
         __syncthreads();
-        // ---- layer 0 and its tangent: H1 = tanh(X W0 + b0); R1 = (1-H1^2) * (X V0 + vb0)
+        // ---- layer 0 and its tangent: H1 = act(X W0 + b0); R1 = act'(H1) * (X V0 + vb0)
         {
             float acc[RM][4], racc[RM][4];
             const float4 bv = *reinterpret_cast<const float4*>(S.P + L::B0 + col0);
@@ -458,15 +477,15 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             for (int i = 0; i < RM; ++i) {
                 float h[4];
 #pragma unroll
-                for (int c = 0; c < 4; ++c) h[c] = tanh_fast(acc[i][c]);
+                for (int c = 0; c < 4; ++c) h[c] = Act::f(acc[i][c]);
                 *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0) = make_float4(h[0], h[1], h[2], h[3]);
                 *reinterpret_cast<float4*>(S.R1 + (row0 + i) * LD + col0) =
-                    make_float4((1.f - h[0] * h[0]) * racc[i][0], (1.f - h[1] * h[1]) * racc[i][1],
-                                (1.f - h[2] * h[2]) * racc[i][2], (1.f - h[3] * h[3]) * racc[i][3]);
+                    make_float4(Act::d(h[0]) * racc[i][0], Act::d(h[1]) * racc[i][1], Act::d(h[2]) * racc[i][2],
+                                Act::d(h[3]) * racc[i][3]);
             }
         }
         __syncthreads();
-        // ---- layer 1 and its tangent: R2 = (1-H2^2) * (R1 W1 + H1 V1 + vb1)
+        // ---- layer 1 and its tangent: R2 = act'(H2) * (R1 W1 + H1 V1 + vb1)
         {
             float acc[RM][4], racc[RM][4];
             const float4 bv = *reinterpret_cast<const float4*>(S.P + L::B1 + col0);
@@ -483,11 +502,11 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             for (int i = 0; i < RM; ++i) {
                 float h[4];
 #pragma unroll
-                for (int c = 0; c < 4; ++c) h[c] = tanh_fast(acc[i][c]);
+                for (int c = 0; c < 4; ++c) h[c] = Act::f(acc[i][c]);
                 *reinterpret_cast<float4*>(S.H2 + (row0 + i) * LD + col0) = make_float4(h[0], h[1], h[2], h[3]);
                 *reinterpret_cast<float4*>(S.R2 + (row0 + i) * LD + col0) =
-                    make_float4((1.f - h[0] * h[0]) * racc[i][0], (1.f - h[1] * h[1]) * racc[i][1],
-                                (1.f - h[2] * h[2]) * racc[i][2], (1.f - h[3] * h[3]) * racc[i][3]);
+                    make_float4(Act::d(h[0]) * racc[i][0], Act::d(h[1]) * racc[i][1], Act::d(h[2]) * racc[i][2],
+                                Act::d(h[3]) * racc[i][3]);
             }
         }
         __syncthreads();
@@ -561,7 +580,8 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             }
         }
         __syncthreads();
-        // ---- D2 = dH2 * g2 -> H2 ; C2 = CdH2 * g2 + ac * dH2 * (-2 H2 R2) -> R2 ; out_b1 accumulates C2 on the fly
+        // ---- D2 = dH2 * g2 -> H2 ; C2 = CdH2 * g2 + ac * dH2 * (act''/act')(H2) R2 -> R2 (g2 = act'(H2); tanh: act''/act' = -2 H2);
+        //      out_b1 accumulates C2 on the fly
 #pragma unroll
         for (int i = 0; i < RM; ++i) {
             const int b = row0 + i;
@@ -579,9 +599,8 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
                     dh = fmaf(dm, w2, dh);
                     ch = fmaf(S.CMU[b * DA + d], w2, fmaf(ac * dm, v2, ch));
                 }
-                const float g2 = 1.f - hv[c] * hv[c];
-                d2[c] = dh * g2;
-                c2[c] = ch * g2 + ac * dh * (-2.f * hv[c] * rv[c]);
+                d2[c] = dh * Act::d(hv[c]);
+                c2[c] = act_hvp_back<Act>(ch, dh, hv[c], rv[c], ac);
                 gB1p[c] += c2[c];
             }
             *reinterpret_cast<float4*>(S.H2 + b * LD + col0) = make_float4(d2[0], d2[1], d2[2], d2[3]);
@@ -605,7 +624,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
         gemm_tile<HID, LD, HID, RM>(S.R2, S.W1T, row0, col0, ch1);
         gemm_tile<HID, LD, HID, RM>(S.H2, S.W1T, row0, col0, dh1);
         __syncthreads();   // all reads of H1 / R1 by the weight-gradient loops are done
-        // ---- C1 = CdH1 * g1 + ac * dH1 * (-2 H1 R1) -> H1 ; out_b0 accumulates C1 on the fly
+        // ---- C1 = CdH1 * g1 + ac * dH1 * (act''/act')(H1) R1 -> H1 ; out_b0 accumulates C1 on the fly
 #pragma unroll
         for (int i = 0; i < RM; ++i) {
             const float4 h4 = *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0);
@@ -614,7 +633,7 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
             float c1[4];
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-                c1[c] = ch1[i][c] * (1.f - hv[c] * hv[c]) + ac * dh1[i][c] * (-2.f * hv[c] * rv[c]);
+                c1[c] = act_hvp_back<Act>(ch1[i][c], dh1[i][c], hv[c], rv[c], ac);
                 gB0p[c] += c1[c];
             }
             *reinterpret_cast<float4*>(S.H1 + (row0 + i) * LD + col0) = make_float4(c1[0], c1[1], c1[2], c1[3]);
@@ -635,12 +654,17 @@ __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) {
     if (cur_m >= 0) flush(cur_m);
 }
 
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) { policy_hvp_body<DO, DA, HID, ActTanh>(A); }
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS) policy_hvp_relu_kernel(PolicyArgs A) { policy_hvp_body<DO, DA, HID, ActRelu>(A); }
+
 // -------------------------------------------------------------------------------------------------
 // forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling).  obs_dim / act_dim: the
 // logical sizes, read only by the padded instantiations (IsBucket)
-template <int DO, int DA, int HID>
-__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride, const float* obs,
-                                                              float* mean, int obs_dim, int act_dim) {
+template <int DO, int DA, int HID, class Act>
+__device__ __forceinline__ void policy_forward_body(int M, int N, const float* params, int64_t stride, const float* obs,
+                                                    float* mean, int obs_dim, int act_dim) {
     using L = PLayout<DO, DA, HID>;
     constexpr bool BUCKET = IsBucket<DO, DA>::value;
     const int dO = BUCKET ? obs_dim : DO, dA = BUCKET ? act_dim : DA;
@@ -658,7 +682,7 @@ __global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const
             const int j = lane + 32 * u;
             float z = sP[L::B0 + j];
             for (int i = 0; i < dO; ++i) z = fmaf(__ldg(o + i), sP[L::W0 + i * HID + j], z);
-            sh[w][j] = tanh_fast(z);
+            sh[w][j] = Act::f(z);
         }
         __syncwarp();
         float mu[DA];
@@ -669,7 +693,7 @@ __global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const
             const int j = lane + 32 * u;
             float z = sP[L::B1 + j];
             for (int k = 0; k < HID; ++k) z = fmaf(sh[w][k], sP[L::W1 + k * HID + j], z);
-            const float h2 = tanh_fast(z);
+            const float h2 = Act::f(z);
 #pragma unroll
             for (int d = 0; d < DA; ++d) mu[d] = fmaf(h2, sP[L::W2 + j * DA + d], mu[d]);
         }
@@ -682,6 +706,18 @@ __global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const
     }
 }
 
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(128) policy_forward_kernel(int M, int N, const float* params, int64_t stride, const float* obs,
+                                                              float* mean, int obs_dim, int act_dim) {
+    policy_forward_body<DO, DA, HID, ActTanh>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+}
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(128) policy_forward_relu_kernel(int M, int N, const float* params, int64_t stride,
+                                                                   const float* obs, float* mean, int obs_dim, int act_dim) {
+    policy_forward_body<DO, DA, HID, ActRelu>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+}
+
+#ifndef PROMP_POLICY_RELU_TU
 __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, float* out) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P) return;
@@ -815,10 +851,18 @@ __global__ void adapt_kl_coeff_kernel(int S1, const float* __restrict__ final_te
     }
 }
 
-// -------------------------------------------------------------------------------------------------
-static int g_use_tc = 1;     // promp_set_option("tensor_cores", 0|1): HID = 64 policy kernels on the tensor cores, 3xTF32 (default) or CUDA cores
+#endif  // !PROMP_POLICY_RELU_TU
 
-static int g_tc_threads = 0;  // promp_set_option("tc_threads", 0|256|512): 0 = per-shape default
+// -------------------------------------------------------------------------------------------------
+// options of promp_set_option, defined by the tanh translation unit and read by both
+#ifdef PROMP_POLICY_RELU_TU
+#define PROMP_OPTION(name, init) extern int name
+#else
+#define PROMP_OPTION(name, init) int name = init
+#endif
+PROMP_OPTION(g_use_tc, 1);     // promp_set_option("tensor_cores", 0|1): HID = 64 policy kernels on the tensor cores, 3xTF32 (default) or CUDA cores
+
+PROMP_OPTION(g_tc_threads, 0);  // promp_set_option("tc_threads", 0|256|512): 0 = per-shape default
 // column groups of the TC kernels' thread mapping: 2 -> 256 threads (32 hidden units per thread), 4 -> 512 threads (16)
 static int tc_column_groups(int obs_dim) {
     if (g_tc_threads == 256) return 2;
@@ -879,50 +923,66 @@ static int launch_policy(Kernel kernel, int smem, int& occ_cache, PolicyArgs& A,
     return PROMP_OK;
 }
 
-template <int DO, int DA, int HID>
+// The kernel of each family for activation Act: policy_*_kernel (tanh) or policy_*_relu_kernel (ReLU).  `if constexpr`
+// names only the selected one, so a tanh launcher instantiates exactly the kernels it did before ReLU existed.
+template <class Act>
+constexpr bool is_relu() { return std::is_same<Act, ActRelu>::value; }
+#define PROMP_ACT_KERNEL(Act, NAME, ...)                                                               \
+    [] {                                                                                               \
+        if constexpr (is_relu<Act>()) return NAME##_relu_kernel<__VA_ARGS__>;                          \
+        else return NAME##_kernel<__VA_ARGS__>;                                                        \
+    }()
+
+template <int DO, int DA, int HID, class Act>
 static int launch_grad(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
     static int occ = 0;
-    return launch_policy(policy_grad_kernel<DO, DA, HID>, (int)sizeof(GradSmem<DO, DA, HID>), occ, A,
-                         PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_kernel");
+    constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_grad, DO, DA, HID);
+    return launch_policy(kernel, (int)sizeof(GradSmem<DO, DA, HID>), occ, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
+                         "policy_grad_kernel");
 }
 
-template <int DO, int DA, int HID>
+template <int DO, int DA, int HID, class Act>
 static int launch_grad_any(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
     if constexpr (HID == TC_HID) {
         if (g_use_tc) {
             static int occ2 = 0, occ4 = 0;
+            constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_grad_tc, DO, DA, 4);
+            constexpr auto k2 = PROMP_ACT_KERNEL(Act, policy_grad_tc, DO, DA, 2);
             if (tc_column_groups(DO) == 4)
-                return launch_policy(policy_grad_tc_kernel<DO, DA, 4>, (int)sizeof(GradTcSmem<DO, DA, 4>), occ4, A,
+                return launch_policy(k4, (int)sizeof(GradTcSmem<DO, DA, 4>), occ4, A,
                                      PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_kernel", TBT, 512);
-            return launch_policy(policy_grad_tc_kernel<DO, DA, 2>, (int)sizeof(GradTcSmem<DO, DA, 2>), occ2, A,
+            return launch_policy(k2, (int)sizeof(GradTcSmem<DO, DA, 2>), occ2, A,
                                  PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_kernel", TBT, 256);
         }
     }
-    return launch_grad<DO, DA, HID>(A, ws, ws_bytes, st);
+    return launch_grad<DO, DA, HID, Act>(A, ws, ws_bytes, st);
 }
 
-template <int DO, int DA, int HID>
+template <int DO, int DA, int HID, class Act>
 static int launch_hvp(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
     if constexpr (HID == TC_HID && sizeof(HvpTcSmem<DO, DA, 2>) <= 227 * 1024) {     // fits the 227 KB of one SM
         if (g_use_tc) {
             static int occ2 = 0, occ4 = 0;
+            constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_hvp_tc, DO, DA, 4);
+            constexpr auto k2 = PROMP_ACT_KERNEL(Act, policy_hvp_tc, DO, DA, 2);
             if (tc_column_groups(DO) == 4)
-                return launch_policy(policy_hvp_tc_kernel<DO, DA, 4>, (int)sizeof(HvpTcSmem<DO, DA, 4>), occ4, A,
+                return launch_policy(k4, (int)sizeof(HvpTcSmem<DO, DA, 4>), occ4, A,
                                      PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_hvp_tc_kernel", TBT, 512);
-            return launch_policy(policy_hvp_tc_kernel<DO, DA, 2>, (int)sizeof(HvpTcSmem<DO, DA, 2>), occ2, A,
+            return launch_policy(k2, (int)sizeof(HvpTcSmem<DO, DA, 2>), occ2, A,
                                  PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_hvp_tc_kernel", TBT, 256);
         }
     }
     static int occ = 0;
-    return launch_policy(policy_hvp_kernel<DO, DA, HID>, (int)sizeof(HvpSmem<DO, DA, HID>), occ, A,
-                         PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_hvp_kernel");
+    constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_hvp, DO, DA, HID);
+    return launch_policy(kernel, (int)sizeof(HvpSmem<DO, DA, HID>), occ, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
+                         "policy_hvp_kernel");
 }
 
 // ---- dataflow chain (policy_chain_tc_kernel): work-item plan + launch ---------------------------------------------
-static int g_chain = -1;         // promp_set_option("chain", -1|0|1): dataflow kernel always (1), never (0: one launch per stage), or
-                                 // where it wins (-1, default; see chain_uses_dataflow)
-static int g_chain_q = 0;        // promp_set_option("chain_q", q): tiles per work item (0 = automatic)
-static int g_chain_taper = 1;    // promp_set_option("chain_taper", 0|1): last stage's items shrink to one tile towards the end
+PROMP_OPTION(g_chain, -1);         // promp_set_option("chain", -1|0|1): dataflow kernel always (1), never (0: one launch per stage),
+                                   // or where it wins (-1, default; see chain_uses_dataflow)
+PROMP_OPTION(g_chain_q, 0);        // promp_set_option("chain_q", q): tiles per work item (0 = automatic)
+PROMP_OPTION(g_chain_taper, 1);    // promp_set_option("chain_taper", 0|1): last stage's items shrink to one tile towards the end
 
 struct ChainPlan {
     ChainStageInfo info[CHAIN_MAX_STAGES];
@@ -998,11 +1058,12 @@ static constexpr bool chain_tc_ok() {
     return false;
 }
 
-template <int DO, int DA, int NQ, bool HAS_HVP>
+template <int DO, int DA, int NQ, bool HAS_HVP, class Act>
 static int launch_chain_nq(ChainArgs& C, cudaStream_t st) {
     static int configured = 0;
     constexpr int smem = ChainSmem<DO, DA, NQ>::SIZE;
-    auto kernel = policy_chain_tc_kernel<DO, DA, NQ, HAS_HVP>;
+    static_assert(std::is_same<Act, ChainAct>::value, "the chain kernel of this translation unit");
+    constexpr auto kernel = PROMP_CHAIN_KERNEL<DO, DA, NQ, HAS_HVP>;
     if (!configured) {
         PROMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = 1;
@@ -1016,7 +1077,7 @@ static int launch_chain_nq(ChainArgs& C, cudaStream_t st) {
 
 // kinds / Ns / A: the stages in order.  Falls back to one launch per stage (same results up to summation order) for the
 // shapes the tensor-core kernels do not cover or when the "chain" option is off.
-template <int DO, int DA, int HID>
+template <int DO, int DA, int HID, class Act>
 static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag, const float* skip_theta, void* ws,
                         int64_t ws_bytes, cudaStream_t st) {
     constexpr int P = PLayout<DO, DA, HID>::P;
@@ -1046,8 +1107,8 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
             bool has_hvp = false;
             for (int s = 0; s < n_stages; ++s) has_hvp = has_hvp || kinds[s] == 1;
             if (tc_column_groups(DO) == 4)
-                return has_hvp ? launch_chain_nq<DO, DA, 4, true>(C, st) : launch_chain_nq<DO, DA, 4, false>(C, st);
-            return has_hvp ? launch_chain_nq<DO, DA, 2, true>(C, st) : launch_chain_nq<DO, DA, 2, false>(C, st);
+                return has_hvp ? launch_chain_nq<DO, DA, 4, true, Act>(C, st) : launch_chain_nq<DO, DA, 4, false, Act>(C, st);
+            return has_hvp ? launch_chain_nq<DO, DA, 2, true, Act>(C, st) : launch_chain_nq<DO, DA, 2, false, Act>(C, st);
         }
     }
     // one launch per stage; their (counters + partial) workspace starts after the chain's control words
@@ -1056,13 +1117,15 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
     for (int s = 0; s < n_stages; ++s) {
         PolicyArgs a = A[s];
         if (s == 0) a.skip_flag = skip_flag, a.skip_theta = skip_theta;
-        const int rc = kinds[s] == 0 ? launch_grad_any<DO, DA, HID>(a, ws1, ws1_bytes, st) : launch_hvp<DO, DA, HID>(a, ws1, ws1_bytes, st);
+        const int rc = kinds[s] == 0 ? launch_grad_any<DO, DA, HID, Act>(a, ws1, ws1_bytes, st)
+                                     : launch_hvp<DO, DA, HID, Act>(a, ws1, ws1_bytes, st);
         if (rc != PROMP_OK) return rc;
     }
     return PROMP_OK;
 }
 
-template <int DO, int DA, int HID>
+// the activation does not change the plan: `Act` only keeps the dispatch uniform
+template <int DO, int DA, int HID, class Act>
 static int chain_num_launches(int n_stages, const int* kinds, const int* Ns, int M) {
     if constexpr (chain_tc_ok<DO, DA, HID>()) {
         const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, PLayout<DO, DA, HID>::P);
@@ -1071,7 +1134,7 @@ static int chain_num_launches(int n_stages, const int* kinds, const int* Ns, int
     return n_stages;
 }
 
-template <int DO, int DA, int HID>
+template <int DO, int DA, int HID, class Act>
 static int64_t chain_ws_bytes(int n_stages, const int* kinds, const int* Ns, int M) {
     const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, PLayout<DO, DA, HID>::P);
     int nmax = 1;
@@ -1080,28 +1143,32 @@ static int64_t chain_ws_bytes(int n_stages, const int* kinds, const int* Ns, int
     return pl.bytes > single ? pl.bytes : single;
 }
 
-template <int DO, int DA, int HID>
+template <int DO, int DA, int HID, class Act>
 static int launch_forward(int M, int N, const float* params, int64_t stride, const float* obs, float* mean, int obs_dim,
                           int act_dim, cudaStream_t st) {
     int gx = (N + 3) / 4;
     const int cap = (4 * sm_count() + M - 1) / M;
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
-    policy_forward_kernel<DO, DA, HID><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+    constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_forward, DO, DA, HID);
+    kernel<<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
     PROMP_LAUNCH_CHECK("policy_forward_kernel");
     return PROMP_OK;
 }
 
+// the instantiation for this translation unit's activation; hid_ = the width decoded from `hidden`
+#define PROMP_DISPATCH_ACT(FN, DO, DA, HID, ...) return FN<DO, DA, HID, PROMP_POLICY_ACT>(__VA_ARGS__);
+
 // supported (obs_dim, act_dim, hidden) instantiations
-#define PROMP_DISPATCH_DIMS(FN, ...)                                                           \
-    if (obs_dim == 2 && act_dim == 2 && hidden == 64) return FN<2, 2, 64>(__VA_ARGS__);        \
-    if (obs_dim == 2 && act_dim == 2 && hidden == 32) return FN<2, 2, 32>(__VA_ARGS__);        \
-    if (obs_dim == 17 && act_dim == 6 && hidden == 64) return FN<17, 6, 64>(__VA_ARGS__);      \
-    if (obs_dim == 17 && act_dim == 6 && hidden == 32) return FN<17, 6, 32>(__VA_ARGS__);      \
-    if (obs_dim == 4 && act_dim == 2 && hidden == 64) return FN<4, 2, 64>(__VA_ARGS__);        \
-    if (obs_dim == 4 && act_dim == 2 && hidden == 32) return FN<4, 2, 32>(__VA_ARGS__);        \
+#define PROMP_DISPATCH_DIMS(FN, ...)                                                                     \
+    if (obs_dim == 2 && act_dim == 2 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 2, 2, 64, __VA_ARGS__)         \
+    if (obs_dim == 2 && act_dim == 2 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 2, 2, 32, __VA_ARGS__)         \
+    if (obs_dim == 17 && act_dim == 6 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 17, 6, 64, __VA_ARGS__)       \
+    if (obs_dim == 17 && act_dim == 6 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 17, 6, 32, __VA_ARGS__)       \
+    if (obs_dim == 4 && act_dim == 2 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 4, 2, 64, __VA_ARGS__)         \
+    if (obs_dim == 4 && act_dim == 2 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 4, 2, 32, __VA_ARGS__)         \
     set_error("unsupported (obs_dim, act_dim, hidden) = (%d, %d, %d); built: (2,2,{32,64}), (4,2,{32,64}), (17,6,{32,64})", \
-              obs_dim, act_dim, hidden);                                                       \
+              obs_dim, act_dim, hidden);                                                                 \
     return PROMP_ERR_INVALID_ARG;
 
 // the padded (bucket) instantiations, at the caps promp_policy_layout gives (obs, act, hidden)
@@ -1109,25 +1176,77 @@ static int launch_forward(int M, int N, const float* params, int64_t stride, con
     {                                                                                                        \
         int32_t lay_[4];                                                                                     \
         if (promp_policy_layout(obs_dim, act_dim, hidden, lay_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;  \
-        if (lay_[0] == 8 && lay_[1] == 2 && hidden == 64) return FN<8, 2, 64>(__VA_ARGS__);                 \
-        if (lay_[0] == 8 && lay_[1] == 2 && hidden == 32) return FN<8, 2, 32>(__VA_ARGS__);                 \
-        if (lay_[0] == 8 && lay_[1] == 8 && hidden == 64) return FN<8, 8, 64>(__VA_ARGS__);                 \
-        if (lay_[0] == 8 && lay_[1] == 8 && hidden == 32) return FN<8, 8, 32>(__VA_ARGS__);                 \
-        if (lay_[0] == 20 && lay_[1] == 2 && hidden == 64) return FN<20, 2, 64>(__VA_ARGS__);               \
-        if (lay_[0] == 20 && lay_[1] == 2 && hidden == 32) return FN<20, 2, 32>(__VA_ARGS__);               \
-        if (lay_[0] == 20 && lay_[1] == 8 && hidden == 64) return FN<20, 8, 64>(__VA_ARGS__);               \
-        if (lay_[0] == 20 && lay_[1] == 8 && hidden == 32) return FN<20, 8, 32>(__VA_ARGS__);               \
-        set_error("no padded instantiation for caps (%d, %d, %d)", lay_[0], lay_[1], hidden);               \
+        if (lay_[0] == 8 && lay_[1] == 2 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 8, 2, 64, __VA_ARGS__)       \
+        if (lay_[0] == 8 && lay_[1] == 2 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 8, 2, 32, __VA_ARGS__)       \
+        if (lay_[0] == 8 && lay_[1] == 8 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 8, 8, 64, __VA_ARGS__)       \
+        if (lay_[0] == 8 && lay_[1] == 8 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 8, 8, 32, __VA_ARGS__)       \
+        if (lay_[0] == 20 && lay_[1] == 2 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 20, 2, 64, __VA_ARGS__)     \
+        if (lay_[0] == 20 && lay_[1] == 2 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 20, 2, 32, __VA_ARGS__)     \
+        if (lay_[0] == 20 && lay_[1] == 8 && hid_ == 64) PROMP_DISPATCH_ACT(FN, 20, 8, 64, __VA_ARGS__)     \
+        if (lay_[0] == 20 && lay_[1] == 8 && hid_ == 32) PROMP_DISPATCH_ACT(FN, 20, 8, 32, __VA_ARGS__)     \
+        set_error("no padded instantiation for caps (%d, %d, %d)", lay_[0], lay_[1], hid_);                 \
         return PROMP_ERR_INVALID_ARG;                                                                        \
     }
 
+// The (obs, act, hidden) dispatch of every entry point for this translation unit's activation: tanh_tu:: here, relu_tu:: in
+// policy_relu.cu.  `hidden` has been checked by decode_hidden; padded = the bucket table of the *_padded entry points.
+namespace PROMP_ACT_NS {
+#define PROMP_DISPATCH(FN, ...)                                                  \
+    const int hid_ = hidden & PROMP_HIDDEN_WIDTH_MASK;                          \
+    if (padded) PROMP_DISPATCH_BUCKETS(FN, __VA_ARGS__)                          \
+    PROMP_DISPATCH_DIMS(FN, __VA_ARGS__)
+int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_grad_any, A, ws, ws_bytes, s)
+}
+int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_hvp, A, ws, ws_bytes, s)
+}
+int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns,
+                              int M) {
+    PROMP_DISPATCH(chain_ws_bytes, n_stages, kinds, Ns, M)
+}
+int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M) {
+    PROMP_DISPATCH(chain_num_launches, n_stages, kinds, Ns, M)
+}
+int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag,
+          const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, ws, ws_bytes, s)
+}
+int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride, const float* obs,
+            float* mean, cudaStream_t s) {
+    PROMP_DISPATCH(launch_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, s)
+}
+}  // namespace PROMP_ACT_NS
+
+#ifndef PROMP_POLICY_RELU_TU
+namespace relu_tu {      // policy_relu.cu
+int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);
+int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);
+int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns,
+                              int M);
+int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M);
+int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag,
+          const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);
+int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride, const float* obs,
+            float* mean, cudaStream_t s);
+}  // namespace relu_tu
+#endif
+
+// checks `hidden` (decode_hidden) and selects the dispatch namespace of its activation; returns from the caller on bad bits
+#define PROMP_DECODE_HIDDEN(who)                                                                 \
+    int hid_ = 0;                                                                                \
+    bool relu_ = false;                                                                          \
+    if (decode_hidden(who, hidden, hid_, relu_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+
 }  // namespace promp
+
+#ifndef PROMP_POLICY_RELU_TU
 
 using namespace promp;
 
 extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int act_dim, int hidden) {
     // upper bound over the occupancies the kernels can have (1..4 CTAs per SM on this device's SMs, or on 160)
-    const int P = promp::num_params(obs_dim, act_dim, hidden);
+    const int P = promp_num_params(obs_dim, act_dim, hidden);
     int64_t worst = 0;
     for (int occ = 1; occ <= 4; ++occ)
         for (int tb : {TB, TBT}) {            // CUDA-core kernels tile by 64 samples, the tensor-core kernels by 128
@@ -1141,6 +1260,10 @@ extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int a
 
 extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]) {
     PROMP_REQUIRE(out != nullptr, "promp_policy_layout: null output");
+    int width;           // the activation does not change the layout
+    bool relu;
+    if (decode_hidden("promp_policy_layout", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    hidden = width;
     PROMP_REQUIRE(obs_dim >= 1 && obs_dim <= 19 && act_dim >= 1 && act_dim <= 8 && (hidden == 32 || hidden == 64),
                   "promp_policy_layout: padded policy kernels take obs_dim in [1, 19], act_dim in [1, 8] and hidden 32 or 64 "
                   "(got %d, %d, %d)", obs_dim, act_dim, hidden);
@@ -1189,8 +1312,8 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
     A.skip_flag = skip_flag; A.skip_theta = skip_theta; A.unclipped_out = unclipped_out; A.theta_copy_out = theta_copy_out;
     A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
-    if (padded) PROMP_DISPATCH_BUCKETS(launch_grad_any, A, workspace, workspace_bytes, s)
-    PROMP_DISPATCH_DIMS(launch_grad_any, A, workspace, workspace_bytes, s)
+    PROMP_DECODE_HIDDEN("promp_policy_grad")
+    return (relu_ ? relu_tu::grad : tanh_tu::grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_GRAD_EX_PARAMS                                                                                               \
@@ -1248,8 +1371,8 @@ static int policy_hvp_impl(bool padded, int obs_dim, int act_dim, int hidden, in
     A.vec = vec; A.out = out; A.inner_lr = inner_lr; A.stats = stats; A.n_valid = n_valid;
     A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
-    if (padded) PROMP_DISPATCH_BUCKETS(launch_hvp, A, workspace, workspace_bytes, s)
-    PROMP_DISPATCH_DIMS(launch_hvp, A, workspace, workspace_bytes, s)
+    PROMP_DECODE_HIDDEN("promp_policy_hvp")
+    return (relu_ ? relu_tu::hvp : tanh_tu::hvp)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_HVP_RAGGED_PARAMS                                                                                            \
@@ -1309,8 +1432,9 @@ static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int a
     if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
-    if (padded) PROMP_DISPATCH_BUCKETS(chain_ws_bytes, n_stages, kinds, Ns, M)
-    PROMP_DISPATCH_DIMS(chain_ws_bytes, n_stages, kinds, Ns, M)
+    PROMP_DECODE_HIDDEN("promp_policy_chain_workspace_bytes")
+    return (relu_ ? relu_tu::chain_workspace_bytes : tanh_tu::chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, n_stages,
+                                                                                      kinds, Ns, M);
 }
 extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                       const promp_policy_stage* stages) {
@@ -1326,8 +1450,8 @@ static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim,
     if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
-    if (padded) PROMP_DISPATCH_BUCKETS(chain_num_launches, n_stages, kinds, Ns, M)
-    PROMP_DISPATCH_DIMS(chain_num_launches, n_stages, kinds, Ns, M)
+    PROMP_DECODE_HIDDEN("promp_policy_chain_num_launches")
+    return (relu_ ? relu_tu::chain_launches : tanh_tu::chain_launches)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
 }
 extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                const promp_policy_stage* stages) {
@@ -1351,8 +1475,9 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
                   "promp_policy_chain: launch re-use is defined for a gradient stage 0 on shared parameters (param_stride 0)");
     for (int k = 0; k < n_stages; ++k) A[k].obs_dim = obs_dim, A[k].act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
-    if (padded) PROMP_DISPATCH_BUCKETS(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, workspace, workspace_bytes, s)
-    PROMP_DISPATCH_DIMS(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, workspace, workspace_bytes, s)
+    PROMP_DECODE_HIDDEN("promp_policy_chain")
+    return (relu_ ? relu_tu::chain : tanh_tu::chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta,
+                                                    workspace, workspace_bytes, s);
 }
 extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
                                   const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
@@ -1400,8 +1525,8 @@ static int policy_forward_impl(bool padded, int obs_dim, int act_dim, int hidden
     PROMP_REQUIRE(M > 0 && N > 0 && params && obs && mean, "promp_policy_forward: bad arguments");
     PROMP_REQUIRE(M <= 65535, "promp_policy_forward: M=%d exceeds the grid.y limit", M);
     cudaStream_t s = (cudaStream_t)stream;
-    if (padded) PROMP_DISPATCH_BUCKETS(launch_forward, M, N, params, param_stride, obs, mean, obs_dim, act_dim, s)
-    PROMP_DISPATCH_DIMS(launch_forward, M, N, params, param_stride, obs, mean, obs_dim, act_dim, s)
+    PROMP_DECODE_HIDDEN("promp_policy_forward")
+    return (relu_ ? relu_tu::forward : tanh_tu::forward)(padded, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, s);
 }
 extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
                                     int64_t param_stride, const float* obs, float* mean, void* stream) {
@@ -1482,3 +1607,4 @@ extern "C" int promp_debug_phase_clocks(unsigned long long* out16, int reset) {
     return 0;
 }
 #endif
+#endif  // !PROMP_POLICY_RELU_TU

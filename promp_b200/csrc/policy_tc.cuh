@@ -314,7 +314,7 @@ __device__ unsigned long long g_phase_clk[16];
 #endif
 // The tile loop of the gradient kernel over the range `sc` describes.  `cached_th` = the parameter vector whose weights
 // the shared-memory tiles currently hold (nullptr: none) - kept across calls by the dataflow kernel.
-template <int DO, int DA, int NQ, class Sched>
+template <int DO, int DA, int NQ, class Act, class Sched>
 __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO, DA, NQ>& S, const Sched& sc,
                                               const float*& cached_th) {
     constexpr int HID = TC_HID;
@@ -484,7 +484,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         }
         __syncthreads();
         PCLK(0);
-        // ---- layer 0 (CUDA cores, row / column-group role): H1 = tanh(X W0 + b0) -> A0
+        // ---- layer 0 (CUDA cores, row / column-group role): H1 = act(X W0 + b0) -> A0
         {
             float x[DO];
 #pragma unroll
@@ -498,7 +498,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     float z = S.Ps[SL::B0 + c];
 #pragma unroll
                     for (int i = 0; i < DO; ++i) z = fmaf(x[i], S.Ps[SL::W0 + i * HID + c], z);
-                    h[e] = tanh_fast(z);
+                    h[e] = Act::f(z);
                 }
                 *reinterpret_cast<float4*>(S.A0 + core_off(r, c0 + 4 * c4, SCA)) = make_float4(h[0], h[1], h[2], h[3]);
             }
@@ -526,7 +526,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int c = 4 * c4 + e;
-                h2[c] = tanh_fast(h2[c] + S.Ps[SL::B1 + c0 + c]);
+                h2[c] = Act::f(h2[c] + S.Ps[SL::B1 + c0 + c]);
 #pragma unroll
                 for (int d = 0; d < DA; ++d) mup[d] = fmaf(h2[c], S.Ps[SL::W2 + (c0 + c) * DA + d], mup[d]);
             }
@@ -600,7 +600,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         }
         __syncthreads();
         PCLK(5);
-        // ---- D2 = (DMU W2^T) * (1 - H2^2) from the h2 registers -> A1
+        // ---- D2 = (DMU W2^T) * act'(H2) from the h2 registers -> A1
         {
             float dm[DA];
 #pragma unroll
@@ -614,7 +614,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     float dh = 0.f;
 #pragma unroll
                     for (int d = 0; d < DA; ++d) dh = fmaf(dm[d], S.Ps[SL::W2 + (c0 + c) * DA + d], dh);
-                    v[e] = dh * (1.f - h2[c] * h2[c]);
+                    v[e] = dh * Act::d(h2[c]);
                 }
                 *reinterpret_cast<float4*>(S.A1 + core_off(r, c0 + 4 * c4, SCA)) = make_float4(v[0], v[1], v[2], v[3]);
             }
@@ -624,7 +624,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
         // ---- weight gradient gW1 += H1^T D2 (mma.sync 3xTF32) and the bias column sums
         wgrad_mma_tile<true, NT, true>(S.A0, S.A1, 1.f, warp, lane, gW1, gB1f);
         PCLK(7);
-        // ---- backward GEMM on the tensor cores: dH1 = D2 W1^T (registers), then D1 = dH1 * (1 - H1^2) -> A0 in place
+        // ---- backward GEMM on the tensor cores: dH1 = D2 W1^T (registers), then D1 = dH1 * act'(H1) -> A0 in place
         {
             float acc[LNT][4];
             zero_frag<LNT>(acc);
@@ -639,7 +639,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                 for (int h = 0; h < 2; ++h) {
                     float2* p = reinterpret_cast<float2*>(S.A0 + frag_off<LNT>(warp, lane, nt, h));
                     const float2 hv = *p;
-                    *p = make_float2(acc[nt][2 * h] * (1.f - hv.x * hv.x), acc[nt][2 * h + 1] * (1.f - hv.y * hv.y));
+                    *p = make_float2(acc[nt][2 * h] * Act::d(hv.x), acc[nt][2 * h + 1] * Act::d(hv.y));
                 }
         }
         __syncthreads();
@@ -670,8 +670,8 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #endif
 }
 
-template <int DO, int DA, int NQ>
-__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs A) {
+template <int DO, int DA, int NQ, class Act>
+__device__ __forceinline__ void policy_grad_tc_body(const PolicyArgs& A) {
     using SM = GradTcSmem<DO, DA, NQ>;
     using L = PLayout<DO, DA, TC_HID>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -680,8 +680,13 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs 
     reuse_produce<L::P, L::LS, DA>(A);
     const UniformSched sc(A.M, A.N, A.q, A.kmax, TBT);
     const float* cached_th = nullptr;
-    grad_tc_tiles<DO, DA, NQ>(A, S, sc, cached_th);
+    grad_tc_tiles<DO, DA, NQ, Act>(A, S, sc, cached_th);
 }
+// one kernel per activation, as in policy.cu: *_kernel = tanh, *_relu_kernel = ReLU
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs A) { policy_grad_tc_body<DO, DA, NQ, ActTanh>(A); }
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_relu_kernel(PolicyArgs A) { policy_grad_tc_body<DO, DA, NQ, ActRelu>(A); }
 
 
 // =================================================================================================================
@@ -715,7 +720,7 @@ struct HvpTcSmem {
 };
 
 // Tile loop of the HVP kernel; same calling convention as grad_tc_tiles.
-template <int DO, int DA, int NQ, class Sched>
+template <int DO, int DA, int NQ, class Act, class Sched>
 __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, DA, NQ>& S, const Sched& sc,
                                              const float*& cached_th) {
     constexpr int HID = TC_HID;
@@ -917,8 +922,8 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                         z = fmaf(x[i], S.Ps[SL::W0 + i * HID + c], z);
                         rz = fmaf(x[i], S.Vs[SL::W0 + i * HID + c], rz);
                     }
-                    h[e] = tanh_fast(z);
-                    r1[e] = (1.f - h[e] * h[e]) * rz;
+                    h[e] = Act::f(z);
+                    r1[e] = Act::d(h[e]) * rz;
                 }
                 const int off = core_off(r, c0 + 4 * c4, SCA);
                 *reinterpret_cast<float4*>(S.H1 + off) = make_float4(h[0], h[1], h[2], h[3]);
@@ -954,8 +959,8 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const int c = 4 * c4 + e;
-                    h2[c] = tanh_fast(h2[c] + S.Ps[SL::B1 + c0 + c]);
-                    r2[c] = (1.f - h2[c] * h2[c]) * (r2[c] + S.Vs[SL::B1 + c0 + c]);
+                    h2[c] = Act::f(h2[c] + S.Ps[SL::B1 + c0 + c]);
+                    r2[c] = Act::d(h2[c]) * (r2[c] + S.Vs[SL::B1 + c0 + c]);
 #pragma unroll
                     for (int d = 0; d < DA; ++d) {
                         const float w2 = S.Ps[SL::W2 + (c0 + c) * DA + d];
@@ -1039,7 +1044,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
             }
         }
         __syncthreads();
-        // ---- D2 = dH2 g2 -> T2a ; C2 = CdH2 g2 + ac dH2 (-2 H2 R2) -> T2b
+        // ---- D2 = dH2 g2 -> T2a ; C2 = CdH2 g2 + ac dH2 (act''/act')(H2) R2 -> T2b   (g2 = act'(H2); tanh: act''/act' = -2 H2)
         {
             float dm[DA], cm[DA];
 #pragma unroll
@@ -1057,9 +1062,8 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                         dh = fmaf(dm[d], w2, dh);
                         ch = fmaf(cm[d], w2, fmaf(ac * dm[d], v2, ch));
                     }
-                    const float g2 = 1.f - h2[c] * h2[c];
-                    d2[e] = dh * g2;
-                    c2[e] = ch * g2 + ac * dh * (-2.f * h2[c] * r2[c]);
+                    d2[e] = dh * Act::d(h2[c]);
+                    c2[e] = act_hvp_back<Act>(ch, dh, h2[c], r2[c], ac);
                 }
                 const int off = core_off(r, c0 + 4 * c4, SCA);
                 *reinterpret_cast<float4*>(S.T2a + off) = make_float4(d2[0], d2[1], d2[2], d2[3]);
@@ -1074,7 +1078,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
             wgrad_mma_tile<false, NT>(S.R1, S.T2a, ac, warp, lane, gW1, unused);
         }
         // ---- backward MMAs: dH1 = D2 W1^T ; CdH1 = C2 W1^T + D2 (ac V1)^T (registers), then
-        //      C1 = CdH1 g1 + ac dH1 (-2 H1 R1) -> H1 in place
+        //      C1 = CdH1 g1 + ac dH1 (act''/act')(H1) R1 -> H1 in place
         {
             float dacc[LNT][4], cacc[LNT][4];
             zero_frag<LNT>(dacc);
@@ -1095,8 +1099,8 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                     const float2 hv = *p;
                     const float2 rv = *reinterpret_cast<const float2*>(S.R1 + off);
                     const float dx = dacc[nt][2 * h], dy = dacc[nt][2 * h + 1];
-                    *p = make_float2(cacc[nt][2 * h] * (1.f - hv.x * hv.x) + ac * dx * (-2.f * hv.x * rv.x),
-                                     cacc[nt][2 * h + 1] * (1.f - hv.y * hv.y) + ac * dy * (-2.f * hv.y * rv.y));
+                    *p = make_float2(act_hvp_back<Act>(cacc[nt][2 * h], dx, hv.x, rv.x, ac),
+                                     act_hvp_back<Act>(cacc[nt][2 * h + 1], dy, hv.y, rv.y, ac));
                 }
         }
         if constexpr (XPRE) {  // D2 (T2a) is dead: bring the observations back for the input-layer gradient
@@ -1126,15 +1130,19 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
     if (cur_m >= 0) flush(cur_m);
 }
 
-template <int DO, int DA, int NQ>
-__global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_kernel(PolicyArgs A) {
+template <int DO, int DA, int NQ, class Act>
+__device__ __forceinline__ void policy_hvp_tc_body(const PolicyArgs& A) {
     using SM = HvpTcSmem<DO, DA, NQ>;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     SM& S = *reinterpret_cast<SM*>(smem_raw);
     const UniformSched sc(A.M, A.N, A.q, A.kmax, TBT);
     const float* cached_th = nullptr;
-    hvp_tc_tiles<DO, DA, NQ>(A, S, sc, cached_th);
+    hvp_tc_tiles<DO, DA, NQ, Act>(A, S, sc, cached_th);
 }
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_kernel(PolicyArgs A) { policy_hvp_tc_body<DO, DA, NQ, ActTanh>(A); }
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_relu_kernel(PolicyArgs A) { policy_hvp_tc_body<DO, DA, NQ, ActRelu>(A); }
 
 // =================================================================================================================
 // Dataflow kernel: the whole gradient chain of one meta-objective evaluation in ONE persistent launch
@@ -1179,8 +1187,19 @@ struct ChainSmem {
     static constexpr int SIZE = BODY + 16;     // + current item
 };
 
+// One chain kernel per translation unit (policy.cu / policy_relu.cu), for that unit's activation: policy_chain_tc_kernel
+// (tanh) or policy_chain_tc_relu_kernel (ReLU).  The body is written in the kernel itself: passed on to a device function
+// by reference, the __grid_constant__ argument changed the tanh kernels' code.
+#ifdef PROMP_POLICY_RELU_TU
+#define PROMP_CHAIN_KERNEL policy_chain_tc_relu_kernel
+using ChainAct = ActRelu;
+#else
+#define PROMP_CHAIN_KERNEL policy_chain_tc_kernel
+using ChainAct = ActTanh;
+#endif
 template <int DO, int DA, int NQ, bool HAS_HVP = true>
-__global__ void __launch_bounds__(128 * NQ, 1) policy_chain_tc_kernel(const __grid_constant__ ChainArgs C) {
+__global__ void __launch_bounds__(128 * NQ, 1) PROMP_CHAIN_KERNEL(const __grid_constant__ ChainArgs C) {
+    using Act = ChainAct;
     using GS = GradTcSmem<DO, DA, NQ>;
     using HS = HvpTcSmem<DO, DA, NQ>;
     using L = PLayout<DO, DA, TC_HID>;
@@ -1228,10 +1247,10 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_chain_tc_kernel(const __gr
         CCLK(0);
         if (!HAS_HVP || I.kind == 0) {
             cached_h = nullptr;
-            grad_tc_tiles<DO, DA, NQ>(C.st[s], G, sc, cached_g);
+            grad_tc_tiles<DO, DA, NQ, Act>(C.st[s], G, sc, cached_g);
         } else if constexpr (HAS_HVP) {
             cached_g = nullptr;
-            hvp_tc_tiles<DO, DA, NQ>(C.st[s], H, sc, cached_h);
+            hvp_tc_tiles<DO, DA, NQ, Act>(C.st[s], H, sc, cached_h);
         }
     }
 #ifdef PROMP_EXP_CLOCKS

@@ -70,7 +70,7 @@ __device__ unsigned long long g_ro_clk[16];
 #define RCLK(i)
 #endif
 
-template <class Env, int HID>
+template <class Env, int HID, class Act>
 __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
     constexpr int DO = Env::DO, DA = Env::DA, SD = Env::SD, TD = Env::TD;
     constexpr int NU = HID / 32;
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
         RCLK(1);
 
         for (int tt = 0; tt < nt; ++tt) {
-            // ---- layer 0: h1 = tanh(obs W0 + b0)           (policies/networks/mlp.py:96-117)
+            // ---- layer 0: h1 = act(obs W0 + b0)            (policies/networks/mlp.py:96-117)
             float ob[DO];
 #pragma unroll
             for (int i = 0; i < DO; ++i) ob[i] = S.obs[i];
@@ -165,13 +165,13 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
                 float z = b0[u];
 #pragma unroll
                 for (int i = 0; i < DO; ++i) z = fmaf(ob[i], w0[i][u], z);
-                S.h1[lane + 32 * u] = tanh_fast(z);
+                S.h1[lane + 32 * u] = Act::f(z);
             }
             // stage obs_t (the observation the action is computed from)
             if (lane < DO) S.st_obs[tt * DO + lane] = S.obs[lane];
             __syncwarp();
             RCLK(2);
-            // ---- layer 1: h2 = tanh(h1 W1 + b1); NACC accumulators per output for ILP (4 where the registers allow it)
+            // ---- layer 1: h2 = act(h1 W1 + b1); NACC accumulators per output for ILP (4 where the registers allow it)
             constexpr int NACC = Env::NACC;
             float acc[NU][NACC];
 #pragma unroll
@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             for (int d = 0; d < DA; ++d) mu[d] = 0.f;
 #pragma unroll
             for (int u = 0; u < NU; ++u) {
-                const float h2 = tanh_fast(NACC == 4 ? (acc[u][0] + acc[u][1]) + (acc[u][2 % NACC] + acc[u][3 % NACC]) : acc[u][0] + acc[u][1]);
+                const float h2 = Act::f(NACC == 4 ? (acc[u][0] + acc[u][1]) + (acc[u][2 % NACC] + acc[u][3 % NACC]) : acc[u][0] + acc[u][1]);
 #pragma unroll
                 for (int d = 0; d < DA; ++d) mu[d] = fmaf(h2, w2[u][d], mu[d]);
             }
@@ -335,12 +335,18 @@ static int with_env(const char* fn, int env_kind, F&& f) {
     return PROMP_ERR_INVALID_ARG;
 }
 
-static int launch_rollout(const char* fn, int env_kind, int hidden, const RolloutArgs& A, cudaStream_t st) {
+// `hidden` as decode_hidden gives it: width 32 or 64, ReLU or tanh
+static int launch_rollout(const char* fn, int env_kind, int width, bool relu, const RolloutArgs& A, cudaStream_t st) {
     const dim3 grid((A.E + RO_WARPS - 1) / RO_WARPS, A.M);
     return with_env(fn, env_kind, [&](auto env) -> int {
         using Env = typename decltype(env)::type;
-        if (hidden == 64) rollout_kernel<Env, 64><<<grid, RO_WARPS * 32, 0, st>>>(A);
-        else rollout_kernel<Env, 32><<<grid, RO_WARPS * 32, 0, st>>>(A);
+        if (relu) {
+            if (width == 64) rollout_kernel<Env, 64, ActRelu><<<grid, RO_WARPS * 32, 0, st>>>(A);
+            else rollout_kernel<Env, 32, ActRelu><<<grid, RO_WARPS * 32, 0, st>>>(A);
+        } else {
+            if (width == 64) rollout_kernel<Env, 64, ActTanh><<<grid, RO_WARPS * 32, 0, st>>>(A);
+            else rollout_kernel<Env, 32, ActTanh><<<grid, RO_WARPS * 32, 0, st>>>(A);
+        }
         PROMP_LAUNCH_CHECK("rollout_kernel");
         return PROMP_OK;
     });
@@ -368,7 +374,10 @@ extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius,
     PROMP_REQUIRE(M <= 65535, "promp_rollout: M=%d exceeds the grid.y limit 65535", M);
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out,
                   "promp_rollout: null pointer argument");
-    PROMP_REQUIRE(hidden == 64 || hidden == 32, "promp_rollout: hidden size %d unsupported (32 or 64)", hidden);
+    int width;
+    bool relu;
+    if (decode_hidden("promp_rollout", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(width == 64 || width == 32, "promp_rollout: hidden size %d unsupported (32 or 64)", width);
     PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "promp_rollout: bad reward_type %d", reward_type);
     PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || info != nullptr,
                   "promp_rollout: cheetah needs the info buffer [2,M,E,H] ([3,M,E,H] for reward_type 1)");
@@ -383,7 +392,7 @@ extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius,
     RolloutArgs A{reward_type, sparse_radius, normalize_actions, M, E, H, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, info, log_std_out,
                   final_state, 0, H};
-    return launch_rollout("promp_rollout", env_kind, hidden, A, (cudaStream_t)stream);
+    return launch_rollout("promp_rollout", env_kind, width, relu, A, (cudaStream_t)stream);
 }
 
 // MetaPointEnv (early `done`, point_env_2d.py:9-59) in the fused kernel: every env slot records a timeline of `timeline_len`
@@ -400,11 +409,14 @@ extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int
     PROMP_REQUIRE(M <= 65535, "promp_rollout_early_term: M=%d exceeds the grid.y limit 65535", M);
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out,
                   "promp_rollout_early_term: null pointer argument");
-    PROMP_REQUIRE(hidden == 64 || hidden == 32, "promp_rollout_early_term: hidden size %d unsupported (32 or 64)", hidden);
+    int width;
+    bool relu;
+    if (decode_hidden("promp_rollout_early_term", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(width == 64 || width == 32, "promp_rollout_early_term: hidden size %d unsupported (32 or 64)", width);
     RolloutArgs A{0, 0.f, normalize_actions, M, E, timeline_len, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
                   nullptr, 1, horizon};
-    return launch_rollout("promp_rollout_early_term", env_kind, hidden, A, (cudaStream_t)stream);
+    return launch_rollout("promp_rollout_early_term", env_kind, width, relu, A, (cudaStream_t)stream);
 }
 
 __global__ void counter_add_kernel(uint64_t* c, uint64_t inc) { *c += inc; }

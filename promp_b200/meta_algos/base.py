@@ -52,7 +52,7 @@ class MAMLAlgo(object):
     def _workspace(self, N):
         import torch
         p = self.policy
-        need = getattr(_lib.load(), p.entries['workspace_bytes'])(self.meta_batch_size, N, p.obs_dim, p.action_dim, p.hidden)
+        need = getattr(_lib.load(), p.entries['workspace_bytes'])(self.meta_batch_size, N, p.obs_dim, p.action_dim, p.hidden_arg)
         if self._ws is None or self._ws.numel() * 4 < need:
             self._ws = torch.zeros((need + 3) // 4, dtype=torch.int32, device=p.device)   # counters start at zero
         return self._ws
@@ -96,7 +96,7 @@ class MAMLAlgo(object):
         n_valid = getattr(phase, 'n_valid', None)           # variable-length paths: per-task sample counts
         skip = (_lib.ptr(reuse[0]), _lib.ptr(reuse[1])) if reuse is not None else (None, None)
         prod = (_lib.ptr(produce[0]), _lib.ptr(produce[1])) if produce is not None else (None, None)
-        _lib.call(p.entries['grad_ex'], p.obs_dim, p.action_dim, p.hidden, self.meta_batch_size, phase.N, _lib.ptr(n_valid),
+        _lib.call(p.entries['grad_ex'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, phase.N, _lib.ptr(n_valid),
                   _lib.ptr(params), stride, _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.adv),
                   _lib.ptr(phase.mean), _lib.ptr(old_ls), per_sample, obj_kind, float(obj_scale), float(clip_eps),
                   float(kl_coeff), int(clip_log_std), float(p.min_log_std), _lib.ptr(grad), _lib.ptr(out_params),
@@ -124,7 +124,7 @@ class MAMLAlgo(object):
         import torch
         p = self.policy
         arr = (_lib.PolicyStage * len(stages))(*stages)
-        need = getattr(_lib.load(), p.entries['chain_workspace_bytes'])(p.obs_dim, p.action_dim, p.hidden, self.meta_batch_size,
+        need = getattr(_lib.load(), p.entries['chain_workspace_bytes'])(p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size,
                                                                         len(stages), ctypes.cast(arr, ctypes.c_void_p))
         if need < 0:
             raise _lib.PrompLibraryError(p.entries['chain_workspace_bytes'] + ": " + _lib.last_error())
@@ -132,7 +132,7 @@ class MAMLAlgo(object):
             self._ws_chain = torch.zeros((need + 3) // 4, dtype=torch.int32, device=p.device)   # control words start at zero
         ws = self._ws_chain
         skip = (_lib.ptr(reuse[0]), _lib.ptr(reuse[1])) if reuse is not None else (None, None)
-        _lib.call(p.entries['chain'], p.obs_dim, p.action_dim, p.hidden, self.meta_batch_size, float(p.min_log_std), len(stages),
+        _lib.call(p.entries['chain'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, float(p.min_log_std), len(stages),
                   ctypes.cast(arr, ctypes.c_void_p), skip[0], skip[1], _lib.ptr(ws), ws.numel() * 4, _lib.stream())
 
     def _hvp(self, phase, params, stride, vec, out, kl_coeff, clip_log_std, stats=None):
@@ -141,7 +141,7 @@ class MAMLAlgo(object):
         full = getattr(phase, 'log_std_full', None)
         old_ls, per_sample = (full, 1) if full is not None else (phase.log_std, 0)
         n_valid = getattr(phase, 'n_valid', None)           # NULL: every task has N valid samples
-        _lib.call(p.entries['hvp_ragged'], p.obs_dim, p.action_dim, p.hidden, self.meta_batch_size, phase.N, _lib.ptr(n_valid),
+        _lib.call(p.entries['hvp_ragged'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, phase.N, _lib.ptr(n_valid),
                   _lib.ptr(params), stride, _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.adv),
                   _lib.ptr(phase.mean), _lib.ptr(old_ls), per_sample, self.inner_obj_kind, float(self.inner_lr),
                   float(kl_coeff), int(clip_log_std), float(p.min_log_std), _lib.ptr(vec), _lib.ptr(out),

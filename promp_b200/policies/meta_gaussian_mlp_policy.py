@@ -26,8 +26,11 @@ MAX_OBS_DIM, MAX_ACTION_DIM = 19, 8
 POLICY_ENTRIES = ('workspace_bytes', 'forward', 'grad_ex', 'hvp_ragged', 'chain', 'chain_workspace_bytes', 'chain_num_launches')
 
 
-def _is_tanh(fn):
-    return fn is None or fn == 'tanh' or getattr(fn, '__name__', '') == 'tanh'
+def _activation_name(fn):
+    """'tanh' or 'relu' for a supported hidden_nonlinearity (a name, or a callable such as tf.tanh / tf.nn.relu / torch.relu
+    / F.relu, recognised by its __name__), else None."""
+    name = 'tanh' if fn is None else (fn if isinstance(fn, str) else getattr(fn, '__name__', None))
+    return name if name in ('tanh', 'relu') else None
 
 
 class MetaGaussianMLPPolicy(object):
@@ -43,20 +46,26 @@ class MetaGaussianMLPPolicy(object):
         if not (1 <= int(obs_dim) <= MAX_OBS_DIM and 1 <= int(action_dim) <= MAX_ACTION_DIM):
             raise NotImplementedError("promp_b200 policy kernels take obs_dim in [1, %d] and action_dim in [1, %d] (got %d, %d)"
                                       % (MAX_OBS_DIM, MAX_ACTION_DIM, int(obs_dim), int(action_dim)))
-        if not _is_tanh(hidden_nonlinearity) or output_nonlinearity is not None:
-            raise NotImplementedError("promp_b200 kernels implement tanh hidden / identity output non-linearities")
+        act = _activation_name(hidden_nonlinearity)
+        if act is None or output_nonlinearity is not None:
+            raise NotImplementedError("promp_b200 kernels implement tanh or relu hidden / identity output non-linearities "
+                                      "(got hidden_nonlinearity=%r, output_nonlinearity=%r)"
+                                      % (hidden_nonlinearity, output_nonlinearity))
         if not learn_std:
             raise NotImplementedError("learn_std=False is not supported (the reference's meta policy graph requires "
                                       "the log_std variable to be trainable, gaussian_mlp_policy.py:174)")
         self._init_args = dict(meta_batch_size=meta_batch_size, obs_dim=int(obs_dim), action_dim=int(action_dim),
                                name=name, hidden_sizes=hidden_sizes, learn_std=learn_std, init_std=init_std,
-                               min_std=min_std)
+                               min_std=min_std, hidden_nonlinearity=act)
         self.meta_batch_size = meta_batch_size
         self.obs_dim, self.action_dim, self.name = int(obs_dim), int(action_dim), name
         # The kernels are instantiated for 32 and 64 hidden units; other widths run zero-padded: a padded unit has
-        # zero incoming and outgoing weights, so it outputs tanh(0) = 0, receives exactly zero gradient (and zero
+        # zero incoming and outgoing weights, so it outputs tanh(0) = relu(0) = 0, receives exactly zero gradient (and zero
         # Hessian-vector product), and therefore stays zero under SGD / Adam / TRPO steps.
         self.hidden_sizes, self.hidden = hidden_sizes, (32 if max(hidden_sizes) <= 32 else 64)
+        self.hidden_nonlinearity = act
+        # the `hidden` argument of every policy / rollout kernel call: the width, plus the activation flag for ReLU
+        self.hidden_arg = self.hidden | (_lib.ACT_RELU if act == 'relu' else 0)
         self.learn_std = learn_std
         self.min_log_std = math.log(min_std)
         self.init_log_std = math.log(init_std)
@@ -204,7 +213,7 @@ class MetaGaussianMLPPolicy(object):
         assert obs.shape[2] == self.obs_dim
         params, stride, clip = self.sampling_params()
         mean = torch.empty(M, E, self.action_dim, dtype=torch.float32, device=self.device)
-        _lib.call(self.entries['forward'], self.obs_dim, self.action_dim, self.hidden, M, E, _lib.ptr(params), stride,
+        _lib.call(self.entries['forward'], self.obs_dim, self.action_dim, self.hidden_arg, M, E, _lib.ptr(params), stride,
                   _lib.ptr(obs.contiguous()), _lib.ptr(mean), _lib.stream())
         pm = params.view(-1, self.num_params) if stride else params.view(1, -1).expand(M, -1)
         ls = pm[:, self._log_std_lo:self._log_std_lo + self.action_dim]
@@ -242,5 +251,6 @@ class MetaGaussianMLPPolicy(object):
         return {'init_args': dict(self._init_args), 'network_params': self.get_param_values()}
 
     def __setstate__(self, state):
-        self.__init__(_skip_param_init=True, **state['init_args'])      # no Xavier draw: loading must not consume np.random
+        # no Xavier draw: loading must not consume np.random; a state saved before the activation was stored is tanh
+        self.__init__(_skip_param_init=True, **state['init_args'])
         self.set_params(state['network_params'])

@@ -116,7 +116,7 @@ class MetaSampler(object):
             phase.info_keys = keys
         self._phase_counter += 1
         _lib.call('promp_rollout', s['env_kind'], s['reward_type'], s['radius'], int(s.get('normalized', False)), M, E, H,
-                  self.policy.hidden,
+                  self.policy.hidden_arg,
                   _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init_state),
                   _lib.ptr(noise), self.seed, self._phase_counter, _lib.ptr(self._phase_counter_dev), clip,
                   float(self.policy.min_log_std),
@@ -251,7 +251,7 @@ class MetaSampler(object):
             init = torch.from_numpy(np.ascontiguousarray(init, dtype=np.float32).reshape(M, E, -1)).to(dev)
         self._injected_noise = self._injected_init = None
         self._phase_counter += 1
-        _lib.call('promp_rollout_early_term', s['env_kind'], int(s.get('normalized', False)), M, E, T, H, self.policy.hidden,
+        _lib.call('promp_rollout_early_term', s['env_kind'], int(s.get('normalized', False)), M, E, T, H, self.policy.hidden_arg,
                   _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init), _lib.ptr(noise), self.seed,
                   self._phase_counter, _lib.ptr(self._phase_counter_dev), clip, float(self.policy.min_log_std), _lib.ptr(tl['obs']),
                   _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']), _lib.ptr(tl['done']), _lib.ptr(phase.log_std),

@@ -1,4 +1,4 @@
-"""A 7-symbol stand-in for `import tensorflow as tf` so that the reference's UNCHANGED driver
+"""An 8-symbol stand-in for `import tensorflow as tf` so that the reference's UNCHANGED driver
 (meta_policy_search/meta_trainer.py:1,55-57,72-76,152) can run on top of promp_b200, whose state lives
 on the GPU rather than in a TF session.  Put promp_b200/tf_shim on sys.path *instead of* TensorFlow.
 Not used by promp_b200 itself."""
@@ -48,3 +48,9 @@ def set_random_seed(seed):
 
 def tanh(x):            # lets run scripts keep passing hidden_nonlinearity=tf.tanh
     raise NotImplementedError("symbolic placeholder: promp_b200 policies evaluate tanh in CUDA")
+
+
+class nn(object):       # tf.nn.relu: lets run scripts pass hidden_nonlinearity=tf.nn.relu
+    @staticmethod
+    def relu(x):
+        raise NotImplementedError("symbolic placeholder: promp_b200 policies evaluate relu in CUDA")
