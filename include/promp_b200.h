@@ -154,10 +154,12 @@ int promp_env_observe(int env_kind, int n_env, const float* state, float* obs, v
  *   from Philox keyed by (env, step, coordinate); task_params [M, 2] select the reward mode).  timeline_len >= 2*horizon - 1
  *   guarantees that promp_paths_finalize finds enough completed samples.
  * promp_paths_finalize: applies the reference's rule to the timelines: t* = first step at which the paths completed so far
- *   hold >= target_samples (= M*E*H) samples; task m keeps the paths completing at steps <= t*, in (step, env index) order
- *   (meta_sampler.py:116-125); unfinished paths are dropped.  Outputs the per-task path table of
+ *   hold >= target_samples (= M*E*H, > 0) samples; task m keeps the paths completing at steps <= t*, in (step, env index)
+ *   order (meta_sampler.py:116-125); unfinished paths are dropped.  Outputs the per-task path table of
  *   promp_process_samples_ragged (path_off [M, max_paths+1], n_paths [M], n_valid [M]; max_paths >= E*timeline_len is always
- *   enough) and the compacted ragged tensors obs/act/mean [M, max_samples, .], rew, done [M, max_samples]
+ *   enough; a task with more paths keeps its first max_paths in that order, and n_valid and the closing and padding offsets
+ *   count only their samples, while cut_out still reports where the rule stopped) and the compacted ragged tensors
+ *   obs/act/mean [M, max_samples, .], rew, done [M, max_samples]
  *   (max_samples >= E*timeline_len).  src_slot / src_start [M, max_paths]: where every path came from.  cut_out int32[2] =
  *   {t*, target reached}.  workspace: promp_paths_workspace_bytes, zero-filled before first use (left zero).
  */

@@ -26,7 +26,8 @@ __global__ void path_hist_kernel(int n_slots, int T, const uint8_t* __restrict__
     }
 }
 
-// cut[0] = t* (T-1 if the target is never reached), cut[1] = 1 if the target was reached; hist is cleared for the next call
+// cut[0] = t* (T-1 if the target is never reached), cut[1] = 1 if the target was reached; all of hist[0..T-1] is cleared for
+// the next call, including the chunks after the one that holds t*
 __global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, int* hist, int* cut) {
     __shared__ long long s_carry;
     __shared__ int s_found;
@@ -36,6 +37,10 @@ __global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, i
     __syncthreads();
     for (int t0 = 0; t0 < T; t0 += 1024) {
         const int t = t0 + tid;
+        if (s_found >= 0) {                               // past the cut's chunk (s_found is block-uniform here): clear only
+            if (t < T) hist[t] = 0;
+            continue;
+        }
         long long v = t < T ? hist[t] : 0;
         if (t < T) hist[t] = 0;
         s_scan[tid] = v;
@@ -51,7 +56,6 @@ __global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, i
         __syncthreads();
         if (tid == 0) s_carry += s_scan[1023];
         __syncthreads();
-        if (s_found >= 0) break;
     }
     if (tid == 0) {
         cut[0] = s_found >= 0 ? s_found : T - 1;
@@ -68,8 +72,8 @@ __global__ void __launch_bounds__(1024) path_table_kernel(int E, int T, int Pmax
     const int m = blockIdx.x, e = threadIdx.x, lane = e & 31, w = e >> 5;
     const int t_star = cut[0];
     __shared__ int s_wcnt[32], s_wlen[32];
-    __shared__ int s_paths, s_samples;
-    if (e == 0) { s_paths = 0; s_samples = 0; }
+    __shared__ int s_paths, s_samples, s_kept;        // s_kept: samples in the first Pmax paths, once a path Pmax-1 exists
+    if (e == 0) { s_paths = 0; s_samples = 0; s_kept = 0; }
     __syncthreads();
     const uint8_t* d = done + ((int64_t)m * E + (e < E ? e : 0)) * T;
     int32_t* po = path_off + (int64_t)m * (Pmax + 1);
@@ -95,9 +99,11 @@ __global__ void __launch_bounds__(1024) path_table_kernel(int E, int T, int Pmax
         if (fin) {
             const int k = s_paths + cb + c - 1;            // path index inside the task
             if (k < Pmax) {
-                po[k] = s_samples + lb + l - len;          // exclusive prefix of the lengths
+                const int off = s_samples + lb + l - len;  // exclusive prefix of the lengths
+                po[k] = off;
                 src_slot[(int64_t)m * Pmax + k] = e;
                 src_start[(int64_t)m * Pmax + k] = start;
+                if (k == Pmax - 1) s_kept = off + len;
             }
             start = t + 1;
         }
@@ -105,11 +111,13 @@ __global__ void __launch_bounds__(1024) path_table_kernel(int E, int T, int Pmax
         if (e == 0) { s_paths += ctot; s_samples += ltot; }
         __syncthreads();
     }
+    // more than Pmax paths: the table keeps the first Pmax of them, and the closing offset / n_valid count only those
     const int np = min(s_paths, Pmax);
-    for (int k = np + e; k <= Pmax; k += blockDim.x) po[k] = s_samples;     // closing offset (and padding entries)
+    const int nv = s_paths > Pmax ? s_kept : s_samples;
+    for (int k = np + e; k <= Pmax; k += blockDim.x) po[k] = nv;            // closing offset (and padding entries)
     if (e == 0) {
         n_paths[m] = np;
-        n_valid[m] = s_samples;
+        n_valid[m] = nv;
     }
 }
 
@@ -158,6 +166,8 @@ extern "C" int promp_paths_finalize(int M, int E, int timeline_len, int max_path
                   "promp_paths_finalize: bad sizes (1 <= E <= 1024)");
     PROMP_REQUIRE(M <= 65535, "promp_paths_finalize: M=%d exceeds the grid.y limit 65535", M);
     PROMP_REQUIRE(max_samples >= E * timeline_len, "promp_paths_finalize: max_samples must cover E * timeline_len samples per task");
+    PROMP_REQUIRE(target_samples > 0, "promp_paths_finalize: target_samples must be positive (got %lld)",
+                  (long long)target_samples);
     PROMP_REQUIRE(t_done && t_obs && t_act && t_mean && t_rew && path_off && n_paths && n_valid && src_slot && src_start && obs &&
                       act && mean && rew && done && cut_out && workspace,
                   "promp_paths_finalize: null pointer argument");

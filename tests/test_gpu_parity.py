@@ -1021,21 +1021,11 @@ def test_fused_early_termination_matches_reference_rule():
                         np.testing.assert_allclose(nxt, s2, atol=2e-6)
     assert done.any() and (done.sum(-1) > 1).any()            # early terminations happened (several paths per slot)
     # ---- host re-statement of the collect-until-enough rule on the same timelines
-    total, n_samples = M * E * H, 0
-    want_paths = [[] for _ in range(M)]
-    start = np.zeros((M, E), dtype=int)
-    t_star = None
-    for t in range(T):
-        for idx in range(M * E):
-            m, e = divmod(idx, E)
-            if done[m, e, t]:
-                want_paths[m].append((e, start[m, e], t + 1 - start[m, e]))
-                n_samples += t + 1 - start[m, e]
-                start[m, e] = t + 1
-        if n_samples >= total:
-            t_star = t
-            break
-    assert t_star is not None
+    from test_paths_finalize import collect_until
+    total = M * E * H
+    rule = collect_until(done, total)
+    assert rule.reached
+    want_paths, t_star = rule.paths, rule.t_star
     cut = ph.cut.cpu().numpy()
     assert cut[0] == t_star and cut[1] == 1
     n_paths, n_valid, off = ph.n_paths_host, ph.n_valid_host, ph.path_off_host

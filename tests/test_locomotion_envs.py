@@ -340,25 +340,6 @@ def test_fused_rollout_matches_oracle(name, hidden):
             np.testing.assert_allclose(obs[:, :, t + 1].reshape(M * E, Do), _obs(name, st), rtol=1e-4, atol=1e-4)
 
 
-def _collect_until_enough(done, H):
-    """The reference's sampling loop (meta_sampler.py:87-137) restated on recorded timelines: step every env, append a
-    path at the step it completes in env order, stop once the completed paths hold >= M*E*H samples."""
-    M, E, T = done.shape
-    paths = [[] for _ in range(M)]
-    start = np.zeros((M, E), dtype=int)
-    n = 0
-    for t in range(T):
-        for idx in range(M * E):
-            m, e = divmod(idx, E)
-            if done[m, e, t]:
-                paths[m].append((e, start[m, e], t + 1 - start[m, e]))
-                n += t + 1 - start[m, e]
-                start[m, e] = t + 1
-        if n >= M * E * H:
-            return paths, t
-    return None, None
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('name', ['walker_vel', 'walker_direc'])
 def test_walker_fused_early_termination(name):
@@ -416,8 +397,10 @@ def test_walker_fused_early_termination(name):
             ts[done[m, :, t]] = 0
     assert n_flip <= 2 and n_fall >= M * E, (n_flip, n_fall)
     # ---- the path table equals the reference rule applied to the same timelines
-    want_paths, t_star = _collect_until_enough(done, H)
-    assert t_star is not None
+    from test_paths_finalize import collect_until
+    rule = collect_until(done, M * E * H)
+    assert rule.reached
+    want_paths, t_star = rule.paths, rule.t_star
     cut = ph.cut.cpu().numpy()
     assert cut[0] == t_star and cut[1] == 1
     n_paths, n_valid, off = ph.n_paths_host, ph.n_valid_host, ph.path_off_host
