@@ -121,6 +121,24 @@ int promp_rollout(int env_kind, int reward_type, float sparse_radius, int normal
                   float* obs, float* act, float* mean, float* rew, uint8_t* done, float* info,
                   float* log_std_out, float* final_state, void* stream);
 
+/*
+ * promp_rollout_ex / promp_rollout_early_term_ex: promp_rollout / promp_rollout_early_term for one rank's shard of a larger
+ * task batch.  task_offset = global index of the shard's first task (rank * M).  It changes only the Philox key of every
+ * env, (task_offset + m) * E + e instead of m * E + e, so action noise, in-kernel reset states and the walker's fall
+ * redraws are the ones the shard's tasks get in one launch over the whole batch (the reference samples every task of the
+ * meta-batch in one process, samplers/meta_sampler.py:59-137).  All buffers stay local ([M, E, ...]).  task_offset = 0 is
+ * the base entry point, bit for bit (the same kernel code).  Rejected: task_offset < 0, (task_offset + M) * E > 2^32 (the
+ * 32-bit env key).
+ */
+int promp_rollout_ex(int env_kind, int reward_type, float sparse_radius, int normalize_actions,
+                     int M, int E, int H, int hidden,
+                     const float* params, int64_t param_stride,
+                     const float* task_params, const float* init_state, const float* noise,
+                     uint64_t seed, uint64_t stream_id, const uint64_t* stream_id_dev,
+                     int clip_reported_log_std, float min_log_std,
+                     float* obs, float* act, float* mean, float* rew, uint8_t* done, float* info,
+                     float* log_std_out, float* final_state, void* stream, int task_offset);
+
 /* *counter += inc on the stream (device-side phase counter for graph-replayed rollouts). */
 int promp_counter_add(uint64_t* counter, uint64_t inc, void* stream);
 
@@ -174,6 +192,31 @@ int promp_paths_finalize(int M, int E, int timeline_len, int max_paths, int max_
                          const float* t_rew, int32_t* path_off, int32_t* n_paths, int32_t* n_valid, int32_t* src_slot,
                          int32_t* src_start, float* obs, float* act, float* mean, float* rew, uint8_t* done, int32_t* cut_out,
                          void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
+ * The cut over a task batch sharded across ranks.  The reference stops when the completed paths of ALL tasks of the
+ * meta-batch hold meta_batch_size*E*H samples (samplers/meta_sampler.py:87-137), so t* is a property of the whole batch,
+ * not of one shard:
+ * promp_rollout_early_term_ex: the shard's timelines, keyed by global env index (see promp_rollout_ex).
+ * promp_paths_histogram: hist[t] += samples of this shard's paths completing at step t (hist int32 [timeline_len], the
+ *   caller zeroes it; the counts add, so the sum over shards - e.g. an all-reduce - is the histogram of the whole batch).
+ * promp_paths_finalize_ex: promp_paths_finalize with hist_in.  hist_in != NULL: t* = first step at which the cumulative
+ *   sum of hist_in reaches target_samples (the global target, world*M*E*H); hist_in is only read and the workspace is
+ *   not touched.  The table and compaction are per task and take this shard's timelines.  hist_in == NULL: exactly
+ *   promp_paths_finalize.
+ */
+int promp_rollout_early_term_ex(int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon, int hidden,
+                                const float* params, int64_t param_stride, const float* task_params, const float* init_state,
+                                const float* noise, uint64_t seed, uint64_t stream_id, const uint64_t* stream_id_dev,
+                                int clip_reported_log_std, float min_log_std, float* obs, float* act, float* mean, float* rew,
+                                uint8_t* done, float* log_std_out, void* stream, int task_offset);
+int promp_paths_histogram(int M, int E, int timeline_len, const uint8_t* t_done, int32_t* hist, void* stream);
+int promp_paths_finalize_ex(int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim, int act_dim,
+                            int64_t target_samples, const int32_t* hist_in, const uint8_t* t_done, const float* t_obs,
+                            const float* t_act, const float* t_mean, const float* t_rew, int32_t* path_off, int32_t* n_paths,
+                            int32_t* n_valid, int32_t* src_slot, int32_t* src_start, float* obs, float* act, float* mean,
+                            float* rew, uint8_t* done, int32_t* cut_out, void* workspace, int64_t workspace_bytes,
+                            void* stream);
 
 /*
  * MetaSampleProcessor.process_samples (samplers/meta_sample_processor.py:8-49 ->

@@ -44,9 +44,16 @@ _SIGNATURES = {
                               c_uint64, _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'promp_rollout_early_term': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, c_uint64, c_uint64,
                                          _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P]),
+    'promp_rollout_ex': (c_int, [c_int, c_int, c_float, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, c_uint64,
+                                 c_uint64, _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int]),
+    'promp_rollout_early_term_ex': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, c_uint64,
+                                            c_uint64, _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, c_int]),
     'promp_paths_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'promp_paths_finalize': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                      _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P]),
+    'promp_paths_histogram': (c_int, [c_int, c_int, c_int, _P, _P, _P]),
+    'promp_paths_finalize_ex': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P, _P, _P, _P, _P, _P,
+                                        _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P]),
     'promp_counter_add': (c_int, [_P, c_uint64, _P]),
     'promp_env_step': (c_int, [c_int, c_int, c_float, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'promp_env_observe': (c_int, [c_int, c_int, _P, _P, _P]),

@@ -26,9 +26,10 @@ __global__ void path_hist_kernel(int n_slots, int T, const uint8_t* __restrict__
     }
 }
 
-// cut[0] = t* (T-1 if the target is never reached), cut[1] = 1 if the target was reached; all of hist[0..T-1] is cleared for
-// the next call, including the chunks after the one that holds t*
-__global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, int* hist, int* cut) {
+// cut[0] = t* (T-1 if the target is never reached), cut[1] = 1 if the target was reached.  clear == hist (the workspace
+// histogram): all of hist[0..T-1] is cleared for the next call, including the chunks after the one that holds t*.
+// clear == NULL (a caller's histogram, promp_paths_finalize_ex): hist is only read.
+__global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, const int* hist, int* clear, int* cut) {
     __shared__ long long s_carry;
     __shared__ int s_found;
     __shared__ long long s_scan[1024];
@@ -38,11 +39,12 @@ __global__ void __launch_bounds__(1024) path_cut_kernel(int T, int64_t target, i
     for (int t0 = 0; t0 < T; t0 += 1024) {
         const int t = t0 + tid;
         if (s_found >= 0) {                               // past the cut's chunk (s_found is block-uniform here): clear only
-            if (t < T) hist[t] = 0;
+            if (!clear) break;
+            if (t < T) clear[t] = 0;
             continue;
         }
         long long v = t < T ? hist[t] : 0;
-        if (t < T) hist[t] = 0;
+        if (clear && t < T) clear[t] = 0;
         s_scan[tid] = v;
         __syncthreads();
         for (int o = 1; o < 1024; o <<= 1) {          // Hillis-Steele inclusive scan
@@ -157,28 +159,44 @@ extern "C" int64_t promp_paths_workspace_bytes(int M, int E, int timeline_len) {
     return ((int64_t)timeline_len + 8) * 4;          // hist [T] (zero on entry, left zero) + cut [2]
 }
 
-extern "C" int promp_paths_finalize(int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim, int act_dim,
-                                    int64_t target_samples, const uint8_t* t_done, const float* t_obs, const float* t_act,
-                                    const float* t_mean, const float* t_rew, int32_t* path_off, int32_t* n_paths, int32_t* n_valid,
-                                    int32_t* src_slot, int32_t* src_start, float* obs, float* act, float* mean, float* rew,
-                                    uint8_t* done, int32_t* cut_out, void* workspace, int64_t workspace_bytes, void* stream) {
+extern "C" int promp_paths_histogram(int M, int E, int timeline_len, const uint8_t* t_done, int32_t* hist, void* stream) {
+    PROMP_REQUIRE(M > 0 && E > 0 && timeline_len > 0, "promp_paths_histogram: sizes must be positive (got %d, %d, %d)", M, E,
+                  timeline_len);
+    PROMP_REQUIRE((int64_t)M * E <= INT32_MAX, "promp_paths_histogram: M * E = %lld env slots exceeds the int32 range",
+                  (long long)M * E);
+    PROMP_REQUIRE(t_done && hist, "promp_paths_histogram: null pointer argument");
+    const int n_slots = M * E;
+    path_hist_kernel<<<(n_slots + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n_slots, timeline_len, t_done, hist);
+    PROMP_LAUNCH_CHECK("path_hist_kernel");
+    return PROMP_OK;
+}
+
+static int paths_finalize(const char* fn, int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim,
+                          int act_dim, int64_t target_samples, const int32_t* hist_in, const uint8_t* t_done, const float* t_obs,
+                          const float* t_act, const float* t_mean, const float* t_rew, int32_t* path_off, int32_t* n_paths,
+                          int32_t* n_valid, int32_t* src_slot, int32_t* src_start, float* obs, float* act, float* mean,
+                          float* rew, uint8_t* done, int32_t* cut_out, void* workspace, int64_t workspace_bytes, void* stream) {
     PROMP_REQUIRE(M > 0 && E > 0 && E <= 1024 && timeline_len > 0 && max_paths > 0 && max_samples > 0,
-                  "promp_paths_finalize: bad sizes (1 <= E <= 1024)");
-    PROMP_REQUIRE(M <= 65535, "promp_paths_finalize: M=%d exceeds the grid.y limit 65535", M);
-    PROMP_REQUIRE(max_samples >= E * timeline_len, "promp_paths_finalize: max_samples must cover E * timeline_len samples per task");
-    PROMP_REQUIRE(target_samples > 0, "promp_paths_finalize: target_samples must be positive (got %lld)",
-                  (long long)target_samples);
+                  "%s: bad sizes (1 <= E <= 1024)", fn);
+    PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
+    PROMP_REQUIRE(max_samples >= E * timeline_len, "%s: max_samples must cover E * timeline_len samples per task", fn);
+    PROMP_REQUIRE(target_samples > 0, "%s: target_samples must be positive (got %lld)", fn, (long long)target_samples);
     PROMP_REQUIRE(t_done && t_obs && t_act && t_mean && t_rew && path_off && n_paths && n_valid && src_slot && src_start && obs &&
                       act && mean && rew && done && cut_out && workspace,
-                  "promp_paths_finalize: null pointer argument");
-    PROMP_REQUIRE(workspace_bytes >= promp_paths_workspace_bytes(M, E, timeline_len), "promp_paths_finalize: workspace too small");
+                  "%s: null pointer argument", fn);
+    PROMP_REQUIRE(workspace_bytes >= promp_paths_workspace_bytes(M, E, timeline_len), "%s: workspace too small", fn);
     cudaStream_t st = (cudaStream_t)stream;
-    int* hist = (int*)workspace;
-    const int n_slots = M * E;
-    path_hist_kernel<<<(n_slots + 127) / 128, 128, 0, st>>>(n_slots, timeline_len, t_done, hist);
-    PROMP_LAUNCH_CHECK("path_hist_kernel");
-    path_cut_kernel<<<1, 1024, 0, st>>>(timeline_len, target_samples, hist, cut_out);
-    PROMP_LAUNCH_CHECK("path_cut_kernel");
+    if (hist_in) {        // counts summed over every shard of the task batch: scanned as given, left as given
+        path_cut_kernel<<<1, 1024, 0, st>>>(timeline_len, target_samples, hist_in, nullptr, cut_out);
+        PROMP_LAUNCH_CHECK("path_cut_kernel");
+    } else {
+        int* hist = (int*)workspace;
+        const int n_slots = M * E;
+        path_hist_kernel<<<(n_slots + 127) / 128, 128, 0, st>>>(n_slots, timeline_len, t_done, hist);
+        PROMP_LAUNCH_CHECK("path_hist_kernel");
+        path_cut_kernel<<<1, 1024, 0, st>>>(timeline_len, target_samples, hist, hist, cut_out);
+        PROMP_LAUNCH_CHECK("path_cut_kernel");
+    }
     const int threads = ((E + 31) / 32) * 32;
     path_table_kernel<<<M, threads, 0, st>>>(E, timeline_len, max_paths, t_done, cut_out, path_off, n_paths, n_valid, src_slot,
                                              src_start);
@@ -187,4 +205,25 @@ extern "C" int promp_paths_finalize(int M, int E, int timeline_len, int max_path
                                                      src_slot, src_start, t_obs, t_act, t_mean, t_rew, obs, act, mean, rew, done);
     PROMP_LAUNCH_CHECK("path_compact_kernel");
     return PROMP_OK;
+}
+
+extern "C" int promp_paths_finalize(int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim, int act_dim,
+                                    int64_t target_samples, const uint8_t* t_done, const float* t_obs, const float* t_act,
+                                    const float* t_mean, const float* t_rew, int32_t* path_off, int32_t* n_paths, int32_t* n_valid,
+                                    int32_t* src_slot, int32_t* src_start, float* obs, float* act, float* mean, float* rew,
+                                    uint8_t* done, int32_t* cut_out, void* workspace, int64_t workspace_bytes, void* stream) {
+    return paths_finalize("promp_paths_finalize", M, E, timeline_len, max_paths, max_samples, obs_dim, act_dim, target_samples,
+                          nullptr, t_done, t_obs, t_act, t_mean, t_rew, path_off, n_paths, n_valid, src_slot, src_start, obs, act,
+                          mean, rew, done, cut_out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int promp_paths_finalize_ex(int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim, int act_dim,
+                                       int64_t target_samples, const int32_t* hist_in, const uint8_t* t_done, const float* t_obs,
+                                       const float* t_act, const float* t_mean, const float* t_rew, int32_t* path_off,
+                                       int32_t* n_paths, int32_t* n_valid, int32_t* src_slot, int32_t* src_start, float* obs,
+                                       float* act, float* mean, float* rew, uint8_t* done, int32_t* cut_out, void* workspace,
+                                       int64_t workspace_bytes, void* stream) {
+    return paths_finalize("promp_paths_finalize_ex", M, E, timeline_len, max_paths, max_samples, obs_dim, act_dim, target_samples,
+                          hist_in, t_done, t_obs, t_act, t_mean, t_rew, path_off, n_paths, n_valid, src_slot, src_start, obs, act,
+                          mean, rew, done, cut_out, workspace, workspace_bytes, stream);
 }

@@ -9,6 +9,8 @@
 // a per-warp shared-memory line with __syncwarp only (no block barriers), the layer-2 reduction is
 // a warp shuffle, the env state lives in registers, and the trajectory record is staged in shared
 // memory for T_CH steps and flushed as coalesced 128-byte float32 rows.
+#include <type_traits>
+
 #include "envs.cuh"
 
 namespace promp {
@@ -39,6 +41,10 @@ struct RolloutArgs {
     // reports done or after `horizon` steps, the slot is reset in-kernel (Philox) and keeps stepping.  0: fixed-horizon mode.
     int early_term;
     int horizon;
+    // task_offset * E, task_offset = global index of task 0 of this launch (a rank's shard of a larger task batch): added
+    // to the env index of the Philox key only, so a shard draws the noise / reset states its tasks get in one launch over
+    // the whole batch
+    uint32_t key_offset;
 };
 
 template <class Env, int HID>
@@ -70,7 +76,9 @@ __device__ unsigned long long g_ro_clk[16];
 #define RCLK(i)
 #endif
 
-template <class Env, int HID, class Act>
+// KEYED: the launch is a shard of a larger task batch (key_offset != 0).  A separate instantiation, so that adding the
+// offset leaves the code of the unsharded kernels as it was (ptxas schedules their step loop differently otherwise).
+template <class Env, int HID, class Act, bool KEYED>
 __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
     constexpr int DO = Env::DO, DA = Env::DA, SD = Env::SD, TD = Env::TD;
     constexpr int NU = HID / 32;
@@ -90,7 +98,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
 #endif
     const float* th = A.params + (int64_t)m * A.param_stride;
     if (A.stream_id_dev) A.stream_id += *A.stream_id_dev;   // device-side phase counter (CUDA-graph replays)
-    const int64_t env_id = (int64_t)m * A.E + e;     // global env index
+    const int64_t env_id = (int64_t)m * A.E + e;     // env index in this launch's buffers
     const int64_t base = env_id * A.H;               // flat sample offset of this env (n = e*H + t)
 
     // ---- weights -> registers (lane owns hidden units j = lane + 32*u)
@@ -121,7 +129,8 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
 #pragma unroll
     for (int i = 0; i < TD; ++i) task[i] = __ldg(A.task_params + (int64_t)m * TD + i);
 
-    const EnvRng rng{(uint32_t)env_id, (uint32_t)A.stream_id, (uint32_t)((A.stream_id >> 32) & 0xffffffu), A.seed};
+    const EnvRng rng{KEYED ? (uint32_t)env_id + A.key_offset : (uint32_t)env_id, (uint32_t)A.stream_id,
+                     (uint32_t)((A.stream_id >> 32) & 0xffffffu), A.seed};
     Env env;
     if (A.init_state) env.load(A.init_state + env_id * SD, lane);
     else env.reset(rng, 0u, 0x52000000u, lane);
@@ -340,13 +349,18 @@ static int launch_rollout(const char* fn, int env_kind, int width, bool relu, co
     const dim3 grid((A.E + RO_WARPS - 1) / RO_WARPS, A.M);
     return with_env(fn, env_kind, [&](auto env) -> int {
         using Env = typename decltype(env)::type;
-        if (relu) {
-            if (width == 64) rollout_kernel<Env, 64, ActRelu><<<grid, RO_WARPS * 32, 0, st>>>(A);
-            else rollout_kernel<Env, 32, ActRelu><<<grid, RO_WARPS * 32, 0, st>>>(A);
-        } else {
-            if (width == 64) rollout_kernel<Env, 64, ActTanh><<<grid, RO_WARPS * 32, 0, st>>>(A);
-            else rollout_kernel<Env, 32, ActTanh><<<grid, RO_WARPS * 32, 0, st>>>(A);
-        }
+        const auto go = [&](auto keyed) {
+            constexpr bool K = decltype(keyed)::value;
+            if (relu) {
+                if (width == 64) rollout_kernel<Env, 64, ActRelu, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                else rollout_kernel<Env, 32, ActRelu, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+            } else {
+                if (width == 64) rollout_kernel<Env, 64, ActTanh, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                else rollout_kernel<Env, 32, ActTanh, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+            }
+        };
+        if (A.key_offset) go(std::true_type{});
+        else go(std::false_type{});
         PROMP_LAUNCH_CHECK("rollout_kernel");
         return PROMP_OK;
     });
@@ -363,6 +377,45 @@ extern "C" int promp_env_task_dim(int env_kind) {
     return with_env("promp_env_task_dim", env_kind, [](auto env) { return decltype(env)::type::TD; });
 }
 
+// The Philox key of an env is its global index (task_offset + m) * E + e, a 32-bit word
+static int check_task_offset(const char* fn, int task_offset, int M, int E) {
+    PROMP_REQUIRE(task_offset >= 0, "%s: task_offset must be >= 0 (got %d)", fn, task_offset);
+    PROMP_REQUIRE(((int64_t)task_offset + M) * E <= ((int64_t)1 << 32),
+                  "%s: (task_offset + M) * E = (%d + %d) * %d exceeds the 32-bit Philox env key", fn, task_offset, M, E);
+    return PROMP_OK;
+}
+
+static int rollout_fixed(const char* fn, int env_kind, int reward_type, float sparse_radius, int normalize_actions, int M, int E,
+                         int H, int hidden, const float* params, int64_t param_stride, const float* task_params,
+                         const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
+                         const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs, float* act,
+                         float* mean, float* rew, uint8_t* done, float* info, float* log_std_out, float* final_state,
+                         void* stream, int task_offset) {
+    PROMP_REQUIRE(M > 0 && E > 0 && H > 0, "%s: M, E, H must be positive (got %d, %d, %d)", fn, M, E, H);
+    PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
+    if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
+    int width;
+    bool relu;
+    if (decode_hidden(fn, hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
+    PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "%s: bad reward_type %d", fn, reward_type);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || info != nullptr,
+                  "%s: cheetah needs the info buffer [2,M,E,H] ([3,M,E,H] for reward_type 1)", fn);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || reward_type == 0 || reward_type == 1,
+                  "%s: cheetah reward_type must be 0 (RandDirec) or 1 (RandVel)", fn);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_POINT_WALLS || reward_type == PROMP_REWARD_DENSE || reward_type == PROMP_REWARD_DENSE_SQUARED,
+                  "%s: the walls env supports reward_type dense / dense_squared", fn);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_SWIMMER || info != nullptr, "%s: the swimmer needs the info buffer [2,M,E,H]", fn);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_SWIMMER || reward_type == 0, "%s: swimmer reward_type must be 0", fn);
+    PROMP_REQUIRE(env_kind != PROMP_ENV_POINT, "%s: MetaPointEnv terminates early (variable-length paths); use the "
+                                               "stepwise sampler (promp_env_step) for it", fn);
+    RolloutArgs A{reward_type, sparse_radius, normalize_actions, M, E, H, params, param_stride, task_params, init_state, noise, seed,
+                  stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, info, log_std_out,
+                  final_state, 0, H, (uint32_t)task_offset * (uint32_t)E};
+    return launch_rollout(fn, env_kind, width, relu, A, (cudaStream_t)stream);
+}
+
 extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius, int normalize_actions, int M, int E, int H,
                              int hidden,
                              const float* params, int64_t param_stride, const float* task_params,
@@ -370,53 +423,65 @@ extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius,
                              const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs, float* act, float* mean,
                              float* rew, uint8_t* done, float* info, float* log_std_out, float* final_state,
                              void* stream) {
-    PROMP_REQUIRE(M > 0 && E > 0 && H > 0, "promp_rollout: M, E, H must be positive (got %d, %d, %d)", M, E, H);
-    PROMP_REQUIRE(M <= 65535, "promp_rollout: M=%d exceeds the grid.y limit 65535", M);
-    PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out,
-                  "promp_rollout: null pointer argument");
-    int width;
-    bool relu;
-    if (decode_hidden("promp_rollout", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
-    PROMP_REQUIRE(width == 64 || width == 32, "promp_rollout: hidden size %d unsupported (32 or 64)", width);
-    PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "promp_rollout: bad reward_type %d", reward_type);
-    PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || info != nullptr,
-                  "promp_rollout: cheetah needs the info buffer [2,M,E,H] ([3,M,E,H] for reward_type 1)");
-    PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || reward_type == 0 || reward_type == 1,
-                  "promp_rollout: cheetah reward_type must be 0 (RandDirec) or 1 (RandVel)");
-    PROMP_REQUIRE(env_kind != PROMP_ENV_POINT_WALLS || reward_type == PROMP_REWARD_DENSE || reward_type == PROMP_REWARD_DENSE_SQUARED,
-                  "promp_rollout: the walls env supports reward_type dense / dense_squared");
-    PROMP_REQUIRE(env_kind != PROMP_ENV_SWIMMER || info != nullptr, "promp_rollout: the swimmer needs the info buffer [2,M,E,H]");
-    PROMP_REQUIRE(env_kind != PROMP_ENV_SWIMMER || reward_type == 0, "promp_rollout: swimmer reward_type must be 0");
-    PROMP_REQUIRE(env_kind != PROMP_ENV_POINT, "promp_rollout: MetaPointEnv terminates early (variable-length paths); use the "
-                                               "stepwise sampler (promp_env_step) for it");
-    RolloutArgs A{reward_type, sparse_radius, normalize_actions, M, E, H, params, param_stride, task_params, init_state, noise, seed,
-                  stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, info, log_std_out,
-                  final_state, 0, H};
-    return launch_rollout("promp_rollout", env_kind, width, relu, A, (cudaStream_t)stream);
+    return rollout_fixed("promp_rollout", env_kind, reward_type, sparse_radius, normalize_actions, M, E, H, hidden, params,
+                         param_stride, task_params, init_state, noise, seed, stream_id, stream_id_dev, clip_reported_log_std,
+                         min_log_std, obs, act, mean, rew, done, info, log_std_out, final_state, stream, 0);
+}
+
+extern "C" int promp_rollout_ex(int env_kind, int reward_type, float sparse_radius, int normalize_actions, int M, int E, int H,
+                                int hidden, const float* params, int64_t param_stride, const float* task_params,
+                                const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
+                                const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs, float* act,
+                                float* mean, float* rew, uint8_t* done, float* info, float* log_std_out, float* final_state,
+                                void* stream, int task_offset) {
+    return rollout_fixed("promp_rollout_ex", env_kind, reward_type, sparse_radius, normalize_actions, M, E, H, hidden, params,
+                         param_stride, task_params, init_state, noise, seed, stream_id, stream_id_dev, clip_reported_log_std,
+                         min_log_std, obs, act, mean, rew, done, info, log_std_out, final_state, stream, task_offset);
 }
 
 // MetaPointEnv (early `done`, point_env_2d.py:9-59) in the fused kernel: every env slot records a timeline of `timeline_len`
 // steps; paths end on done / after `horizon` steps and the slot is reset in-kernel.  promp_paths_finalize then applies the
 // reference's collect-until-enough rule (meta_sampler.py:87-137) to the timelines.
+static int rollout_early_term(const char* fn, int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon,
+                              int hidden, const float* params, int64_t param_stride, const float* task_params,
+                              const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
+                              const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs, float* act,
+                              float* mean, float* rew, uint8_t* done, float* log_std_out, void* stream, int task_offset) {
+    PROMP_REQUIRE(env_kind == PROMP_ENV_POINT || env_kind == PROMP_ENV_WALKER,
+                  "%s: implemented for MetaPointEnv and the walker (env_kind %d given)", fn, env_kind);
+    PROMP_REQUIRE(M > 0 && E > 0 && timeline_len > 0 && horizon > 0, "%s: sizes must be positive", fn);
+    PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
+    if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
+    int width;
+    bool relu;
+    if (decode_hidden(fn, hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
+    RolloutArgs A{0, 0.f, normalize_actions, M, E, timeline_len, params, param_stride, task_params, init_state, noise, seed,
+                  stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
+                  nullptr, 1, horizon, (uint32_t)task_offset * (uint32_t)E};
+    return launch_rollout(fn, env_kind, width, relu, A, (cudaStream_t)stream);
+}
+
 extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon, int hidden,
                                         const float* params, int64_t param_stride, const float* task_params,
                                         const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
                                         const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std, float* obs,
                                         float* act, float* mean, float* rew, uint8_t* done, float* log_std_out, void* stream) {
-    PROMP_REQUIRE(env_kind == PROMP_ENV_POINT || env_kind == PROMP_ENV_WALKER,
-                  "promp_rollout_early_term: implemented for MetaPointEnv and the walker (env_kind %d given)", env_kind);
-    PROMP_REQUIRE(M > 0 && E > 0 && timeline_len > 0 && horizon > 0, "promp_rollout_early_term: sizes must be positive");
-    PROMP_REQUIRE(M <= 65535, "promp_rollout_early_term: M=%d exceeds the grid.y limit 65535", M);
-    PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out,
-                  "promp_rollout_early_term: null pointer argument");
-    int width;
-    bool relu;
-    if (decode_hidden("promp_rollout_early_term", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
-    PROMP_REQUIRE(width == 64 || width == 32, "promp_rollout_early_term: hidden size %d unsupported (32 or 64)", width);
-    RolloutArgs A{0, 0.f, normalize_actions, M, E, timeline_len, params, param_stride, task_params, init_state, noise, seed,
-                  stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
-                  nullptr, 1, horizon};
-    return launch_rollout("promp_rollout_early_term", env_kind, width, relu, A, (cudaStream_t)stream);
+    return rollout_early_term("promp_rollout_early_term", env_kind, normalize_actions, M, E, timeline_len, horizon, hidden, params,
+                              param_stride, task_params, init_state, noise, seed, stream_id, stream_id_dev, clip_reported_log_std,
+                              min_log_std, obs, act, mean, rew, done, log_std_out, stream, 0);
+}
+
+extern "C" int promp_rollout_early_term_ex(int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon,
+                                           int hidden, const float* params, int64_t param_stride, const float* task_params,
+                                           const float* init_state, const float* noise, uint64_t seed, uint64_t stream_id,
+                                           const uint64_t* stream_id_dev, int clip_reported_log_std, float min_log_std,
+                                           float* obs, float* act, float* mean, float* rew, uint8_t* done, float* log_std_out,
+                                           void* stream, int task_offset) {
+    return rollout_early_term("promp_rollout_early_term_ex", env_kind, normalize_actions, M, E, timeline_len, horizon, hidden,
+                              params, param_stride, task_params, init_state, noise, seed, stream_id, stream_id_dev,
+                              clip_reported_log_std, min_log_std, obs, act, mean, rew, done, log_std_out, stream, task_offset);
 }
 
 __global__ void counter_add_kernel(uint64_t* c, uint64_t inc) { *c += inc; }

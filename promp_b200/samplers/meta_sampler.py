@@ -14,7 +14,7 @@ from promp_b200 import _lib
 from promp_b200.samplers.device_data import (PhaseData, LazyPath, LazyPathList, PathsMetaBatch, DeviceRaggedPhaseData,
                                               RaggedLazyPathList)
 from promp_b200.samplers.vectorized_env_executor import MetaDeviceEnvExecutor
-from promp_b200.utils import logger
+from promp_b200.utils import dist, logger
 from promp_b200.utils.dist import shard_tasks
 
 
@@ -28,7 +28,14 @@ class MetaSampler(object):
             states in-kernel with Philox (nothing crosses PCIe).
         seed (int): Philox key for in-kernel action noise / reset states.
         task_shard ((rank, world)): this process owns tasks [rank*M, (rank+1)*M) of a global batch of
-            world*M tasks; every rank draws the same global task list and keeps its slice.
+            world*M tasks; every rank draws the same global task list and keeps its slice.  On the fused paths a
+            sharded run samples exactly what one process with the global batch samples for the same seeds: the rollout
+            kernels key their Philox streams by the global env index (task offset rank*M), reset_mode='numpy' draws
+            the global batch's reset states and keeps this rank's rows, and early-terminating envs (reset_mode='device')
+            cut their timelines where the completed paths of ALL ranks' tasks reach world*M*E*H samples (the per-step
+            histogram is summed over ranks with utils.dist.allreduce_sum_).  Not covered: the step loop over
+            promp_env_step (early-terminating envs with reset_mode='numpy') and duck-typed host envs reset envs one at
+            a time from the host stream, so their reset draws stay per rank.
     `parallel` is accepted and ignored: there are no env worker processes on the device path.
     """
 
@@ -48,6 +55,9 @@ class MetaSampler(object):
         self.reset_mode = reset_mode
         self.seed = int(seed)
         self.task_shard = task_shard
+        # world > 1: global index of this rank's first task (Philox key offset) and the number of ranks
+        self._shard_world = int(task_shard[1]) if task_shard is not None else 1
+        self._task_offset = int(task_shard[0]) * meta_batch_size if self._shard_world > 1 else 0
         self._phase_counter = 0
         self._phase_counter_dev = None      # device uint64 phase counter (graph mode)
         self._injected_noise = None
@@ -115,13 +125,16 @@ class MetaSampler(object):
             phase.info = torch.empty(len(keys), M, E * H, dtype=torch.float32, device=self.device)
             phase.info_keys = keys
         self._phase_counter += 1
-        _lib.call('promp_rollout', s['env_kind'], s['reward_type'], s['radius'], int(s.get('normalized', False)), M, E, H,
-                  self.policy.hidden_arg,
-                  _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init_state),
-                  _lib.ptr(noise), self.seed, self._phase_counter, _lib.ptr(self._phase_counter_dev), clip,
-                  float(self.policy.min_log_std),
-                  _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.mean), _lib.ptr(phase.rew),
-                  _lib.ptr(phase.done), _lib.ptr(phase.info), _lib.ptr(phase.log_std), None, _lib.stream())
+        args = (s['env_kind'], s['reward_type'], s['radius'], int(s.get('normalized', False)), M, E, H, self.policy.hidden_arg,
+                _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init_state),
+                _lib.ptr(noise), self.seed, self._phase_counter, _lib.ptr(self._phase_counter_dev), clip,
+                float(self.policy.min_log_std),
+                _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.mean), _lib.ptr(phase.rew),
+                _lib.ptr(phase.done), _lib.ptr(phase.info), _lib.ptr(phase.log_std), None, _lib.stream())
+        if self._shard_world > 1:
+            _lib.call('promp_rollout_ex', *args, self._task_offset)
+        else:
+            _lib.call('promp_rollout', *args)
         if self._phase_counter_dev is not None:
             _lib.call('promp_counter_add', _lib.ptr(self._phase_counter_dev), 1 << 20, _lib.stream())
         phase.invalidate_host()
@@ -133,6 +146,15 @@ class MetaSampler(object):
             return self.env.sample_tasks(self.meta_batch_size)
         rank, world = self.task_shard
         return shard_tasks(self.env.sample_tasks(self.meta_batch_size * world), rank, world)
+
+    def _host_reset_states(self, inner, n):
+        """n = M*E reset states from the global numpy RNG for this rank: a sharded run draws the global batch's
+        world*M*E states (the draws are vectorised per coordinate block, so a local draw is not a slice of the global
+        one) and keeps its rows, so that the values and the stream position match a one-process run."""
+        if self._shard_world == 1:
+            return inner.host_reset_states(n)
+        r0 = self.task_shard[0] * n
+        return inner.host_reset_states(self._shard_world * n)[r0:r0 + n]
 
     def draw_host_inputs(self, n_phases, slot=0):
         """Graph mode with reset_mode='numpy', host half: draw one iteration's tasks and every phase's reset states from
@@ -165,8 +187,9 @@ class MetaSampler(object):
         self._staged_tasks[slot] = list(tasks)
         self._pinned_tasks[slot].copy_(torch.from_numpy(np.stack([inner.task_vector(t) for t in tasks]).astype(np.float32)))
         for s in range(n_phases):
-            self._pinned_init[slot][s].copy_(torch.from_numpy(inner.host_reset_states(M * E).astype(np.float32).reshape(M, E, sd)))
-            inner.host_reset_states(M * E)     # discarded end-of-horizon resets (vectorized_env_executor.py:47-50)
+            self._pinned_init[slot][s].copy_(torch.from_numpy(self._host_reset_states(inner, M * E).astype(np.float32)
+                                                              .reshape(M, E, sd)))
+            self._host_reset_states(inner, M * E)     # discarded end-of-horizon resets (vectorized_env_executor.py:47-50)
 
     def upload_host_inputs(self, slot=0):
         """Device half: start the H2D copies of a drawn slot into the static buffers the captured rollouts read."""
@@ -203,7 +226,7 @@ class MetaSampler(object):
         init = self._injected_init
         if init is None and self.reset_mode == 'numpy':
             # vec_env.reset(): M*E reset draws in env order (vectorized_env_executor.py:73)
-            init = inner.host_reset_states(M * E).astype(np.float32)
+            init = self._host_reset_states(inner, M * E).astype(np.float32)
         if init is not None and not isinstance(init, torch.Tensor):
             init = torch.from_numpy(np.ascontiguousarray(init, dtype=np.float32).reshape(M, E, -1)).to(self.device, non_blocking=True)
         noise = self._injected_noise
@@ -214,7 +237,7 @@ class MetaSampler(object):
         if self._injected_init is None and self.reset_mode == 'numpy':
             # at ts == H every env is reset once more and that observation is discarded
             # (vectorized_env_executor.py:47-50): consume the same draws to stay aligned with the reference
-            inner.host_reset_states(M * E)
+            self._host_reset_states(inner, M * E)
         self._injected_noise = self._injected_init = None
         paths = PathsMetaBatch()
         cache = {}
@@ -251,16 +274,33 @@ class MetaSampler(object):
             init = torch.from_numpy(np.ascontiguousarray(init, dtype=np.float32).reshape(M, E, -1)).to(dev)
         self._injected_noise = self._injected_init = None
         self._phase_counter += 1
-        _lib.call('promp_rollout_early_term', s['env_kind'], int(s.get('normalized', False)), M, E, T, H, self.policy.hidden_arg,
-                  _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init), _lib.ptr(noise), self.seed,
-                  self._phase_counter, _lib.ptr(self._phase_counter_dev), clip, float(self.policy.min_log_std), _lib.ptr(tl['obs']),
-                  _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']), _lib.ptr(tl['done']), _lib.ptr(phase.log_std),
-                  _lib.stream())
-        _lib.call('promp_paths_finalize', M, E, T, E * T, n_alloc, Do, Da, M * E * H, _lib.ptr(tl['done']), _lib.ptr(tl['obs']),
-                  _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']), _lib.ptr(phase.path_off), _lib.ptr(phase.n_paths),
-                  _lib.ptr(phase.n_valid), _lib.ptr(phase.src_slot), _lib.ptr(phase.src_start), _lib.ptr(phase.obs), _lib.ptr(phase.act),
-                  _lib.ptr(phase.mean), _lib.ptr(phase.rew), _lib.ptr(phase.done), _lib.ptr(phase.cut), _lib.ptr(tl['ws']),
-                  tl['ws'].numel() * 4, _lib.stream())
+        args = (s['env_kind'], int(s.get('normalized', False)), M, E, T, H, self.policy.hidden_arg,
+                _lib.ptr(params), stride, _lib.ptr(self.vec_env.task_params_per_task), _lib.ptr(init), _lib.ptr(noise), self.seed,
+                self._phase_counter, _lib.ptr(self._phase_counter_dev), clip, float(self.policy.min_log_std), _lib.ptr(tl['obs']),
+                _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']), _lib.ptr(tl['done']), _lib.ptr(phase.log_std),
+                _lib.stream())
+        if self._shard_world > 1:
+            _lib.call('promp_rollout_early_term_ex', *args, self._task_offset)
+        else:
+            _lib.call('promp_rollout_early_term', *args)
+        head = (M, E, T, E * T, n_alloc, Do, Da)
+        tail = (_lib.ptr(tl['done']), _lib.ptr(tl['obs']), _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']),
+                _lib.ptr(phase.path_off), _lib.ptr(phase.n_paths), _lib.ptr(phase.n_valid), _lib.ptr(phase.src_slot),
+                _lib.ptr(phase.src_start), _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.mean), _lib.ptr(phase.rew),
+                _lib.ptr(phase.done), _lib.ptr(phase.cut), _lib.ptr(tl['ws']), tl['ws'].numel() * 4, _lib.stream())
+        if self._shard_world > 1:
+            # the reference's rule over the WHOLE task batch (meta_sampler.py:87-137): t* is the first step at which the
+            # completed paths of every rank's tasks hold world*M*E*H samples, so the per-step counts are summed over ranks
+            # (int32: NCCL) before the cut
+            hist = getattr(self, '_shard_hist', None)
+            if hist is None:
+                hist = self._shard_hist = torch.empty(T, dtype=torch.int32, device=dev)
+            hist.zero_()
+            _lib.call('promp_paths_histogram', M, E, T, _lib.ptr(tl['done']), _lib.ptr(hist), _lib.stream())
+            dist.allreduce_sum_(hist)
+            _lib.call('promp_paths_finalize_ex', *head, self._shard_world * M * E * H, _lib.ptr(hist), *tail)
+        else:
+            _lib.call('promp_paths_finalize', *head, M * E * H, *tail)
         phase.timeline = tl                 # kept for diagnostics / tests (overwritten by the next phase)
         phase.invalidate_host()
         paths = PathsMetaBatch()

@@ -94,7 +94,10 @@ def rank():
 
 def shard_tasks(all_tasks, rank, world):
     """Rank `rank` of `world` owns the contiguous slice of the global task list (every rank draws the same
-    list from the same numpy seed, so results do not depend on the number of GPUs)."""
+    list from the same numpy seed, so every rank gets the tasks a one-GPU run gives it).  With the fused samplers
+    the samples do not depend on the number of GPUs either (MetaSampler: global Philox keys and reset draws, the
+    early-termination cut over all ranks); the step loop over host-reset envs keeps per-rank reset draws, and the
+    meta-gradient all-reduce sums in a rank-dependent order (last-bit differences)."""
     n = len(all_tasks)
     assert n % world == 0, "global meta batch must be divisible by the number of ranks"
     per = n // world
