@@ -56,7 +56,9 @@ enum {
     PROMP_OBJ_RATIO = 0,   /* -mean(ratio*adv)                       meta_algos/pro_mp.py:59-65          */
     PROMP_OBJ_LOGLIK = 1,  /* -mean(logp*adv)                        meta_algos/trpo_maml.py:58-62       */
     PROMP_OBJ_CLIP = 2,    /* -mean(min(r*adv, clip(r,1-e,1+e)*adv)) meta_algos/pro_mp.py:135-141        */
-    PROMP_OBJ_NONE = 3     /* only the kl_coeff * mean KL(old||new) term                                 */
+    PROMP_OBJ_NONE = 3,    /* only the kl_coeff * mean KL(old||new) term                                 */
+    PROMP_OBJ_EXPLORE = 4  /* -c_m * mean(logp): E-MAML exploration term, trpo_maml.py:137-144; `adv` is  */
+                           /* the per-task coefficient c [M] (promp_emaml_coeff), gradient stages only    */
 };
 /* Hidden non-linearity of the policy (policies/networks/mlp.py: hidden_nonlinearity), carried in the `hidden` argument of
  * the policy and rollout entry points: hidden = width | flag, width 32 or 64 in the low byte.  No flag = tanh, so a plain
@@ -338,6 +340,20 @@ int promp_trpo_select(int n, int n_candidates, int n_terms, int k0, int max_back
 int promp_adj_avg_rewards(int64_t n, const float* rew, double mean, double std, float* out, void* stream);
 
 /*
+ * E-MAML coefficient (trpo_maml.py:137-144 with samplers/meta_sample_processor.py:40-44): the task mean of adj_avg_rewards,
+ *   c_m = (mean_m r - mean_all) / (std_all + 1e-8),   mean / std over the rewards of every task (population std),
+ * from the per-task sums stats[m][5] = sum r, stats[m][6] = sum r^2 of promp_process_samples(_ragged) ([M,8] float64).
+ * Every mean covers a task's valid samples: n_m = n_valid[m] ([M] int32 device memory) or N when n_valid is NULL.
+ * Totals are float64 sums in task order; c is written as float32 [M].  One launch, no host arithmetic (capturable).
+ * Several ranks: promp_emaml_totals writes this rank's [sum r, sum r^2, sum n] (float64 [3]); sum them over ranks, then
+ * promp_emaml_finish computes c from the summed totals.
+ */
+int promp_emaml_coeff(int M, const double* stats, const int32_t* n_valid, int N, float* coeff, void* stream);
+int promp_emaml_totals(int M, const double* stats, const int32_t* n_valid, int N, double* totals, void* stream);
+int promp_emaml_finish(int M, const double* stats, const int32_t* n_valid, int N, const double* totals, float* coeff,
+                       void* stream);
+
+/*
  * Per-task objective value, KL and gradient w.r.t. the task's parameter set, optionally fused with
  * the inner SGD step.  Covers
  *   - MAMLAlgo._adapt        (meta_algos/base.py:217-242, graph :158-215): obj RATIO|LOGLIK,
@@ -349,6 +365,7 @@ int promp_adj_avg_rewards(int64_t n, const float* rew, double mean, double std, 
  *                            (policies/distributions/diagonal_gaussian.py:16-109)
  *   - forward_mlp            (policies/networks/mlp.py:65-119)
  * Objective_m = obj_scale * surr_kind(m) + kl_coeff * mean_n KL(old || new)(m).
+ * obj_kind PROMP_OBJ_EXPLORE: adv is [M], one weight per task (the E-MAML coefficient), and the objective is LOGLIK's.
  *
  *   obs [M,N,Do] act [M,N,Da] adv [M,N] old_mean [M,N,Da]
  *   old_log_std: [M,Da] if ls_per_sample == 0 else [M,N,Da]
@@ -441,7 +458,8 @@ typedef struct {
     const float* params;
     int64_t param_stride;
     const float *obs, *act, *adv, *old_mean, *old_log_std;
-    int32_t ls_per_sample, obj_kind;
+    int32_t ls_per_sample, obj_kind;   /* PROMP_OBJ_EXPLORE: last stage only, param_stride 0, no out_params; its items
+                                          wait for no other stage */
     float obj_scale, clip_eps, kl_coeff;
     int32_t clip_log_std;
     float* grad;                   /* gradient stage */
@@ -482,6 +500,9 @@ int promp_meta_loss_terms(int S, int M, const float* stats_all, float inv_m_glob
 
 /* out[P] = scale * sum_m in[m,P]   (mean over tasks of the meta objective, pro_mp.py:151-155). */
 int promp_reduce_tasks(int M, int P, const float* in, float scale, float* out, void* stream);
+/* out[P] = scale * sum_m a[m,P] + scale * sum_m b[m,P]: the meta-gradient plus the E-MAML exploration gradient, equal bit for
+ * bit to promp_reduce_tasks on each and an add. */
+int promp_reduce_tasks2(int M, int P, const float* a, const float* b, float scale, float* out, void* stream);
 
 /*
  * Logged scalars without a host round trip per value (the Trainer reads ONE float64 vector back per iteration):

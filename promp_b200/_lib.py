@@ -17,7 +17,7 @@ ENV_WALKER, ENV_SWIMMER = 5, 6
 EARLY_TERM_ENVS = (ENV_POINT, ENV_WALKER)        # env kinds whose paths end on `done` (variable-length paths)
 INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write env_infos channels
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
-OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE = 0, 1, 2, 3
+OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE, OBJ_EXPLORE = 0, 1, 2, 3, 4
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE = 0, 1
 # the policy / rollout `hidden` argument: width | activation flag (no flag = tanh)
 HIDDEN_WIDTH_MASK, ACT_RELU = 0xFF, 0x100
@@ -65,6 +65,9 @@ _SIGNATURES = {
                                              c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P]),
     'promp_process_launch_info': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'promp_adj_avg_rewards': (c_int, [c_int64, _P, c_double, c_double, _P, _P]),
+    'promp_emaml_coeff': (c_int, [c_int, _P, _P, c_int, _P, _P]),
+    'promp_emaml_totals': (c_int, [c_int, _P, _P, c_int, _P, _P]),
+    'promp_emaml_finish': (c_int, [c_int, _P, _P, c_int, _P, _P, _P]),
     'promp_baseline_fit_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'promp_baseline_fit': (c_int, [c_int, c_int, c_int, _P, _P, _P, c_double, _P, _P, _P, c_int64, _P]),
     'promp_baseline_predict': (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P]),
@@ -87,6 +90,7 @@ _SIGNATURES = {
     'promp_promp_log_terms': (c_int, [c_int, _P, _P, _P]),
     'promp_adapt_kl_coeff': (c_int, [c_int, _P, c_double, c_int, _P, _P, _P]),
     'promp_reduce_tasks': (c_int, [c_int, c_int, _P, c_float, _P, _P]),
+    'promp_reduce_tasks2': (c_int, [c_int, c_int, _P, _P, c_float, _P, _P]),
     'promp_adam_tf1': (c_int, [c_int, _P, _P, _P, _P, _P, c_float, c_float, c_float, c_float, _P]),
     'promp_vec_axpy': (c_int, [c_int, c_float, _P, _P, _P, _P]),
     'promp_cg_init': (c_int, [c_int, _P, _P, _P, _P, _P, _P]),

@@ -45,6 +45,8 @@ struct PolicyArgs {
     const float* vec;
     float* out;
     float inner_lr;
+    int adv_per_task;    // PROMP_OBJ_EXPLORE: adv is a per-task [M] vector (the E-MAML coefficient), obj_kind is LOGLIK.  Read
+                         // only by the *_explore instantiations; it sits in what was alignment padding, like obs_dim.
     float* stats;
     float* partial;      // [grid][kmax][P + PSTAT] per-(CTA, task-segment) partial sums
     int* counters;       // [M], zero on entry, left zero on exit
@@ -64,8 +66,14 @@ struct PolicyArgs {
     // iteration has no host decision: promp_adapt_kl_coeff updates it between launches)
     const float* kl_coeff_ptr;
 };
-static_assert(sizeof(PolicyArgs) == 224 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120,
+static_assert(sizeof(PolicyArgs) == 224 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120 &&
+                  offsetof(PolicyArgs, stats) == 144,
               "PolicyArgs layout");
+
+// Where a kernel reads a sample's advantage: ADV_SAMPLE = adv[n] (every instantiation that existed before the E-MAML
+// objective, unchanged), ADV_TASK = adv[m] (the stand-alone PROMP_OBJ_EXPLORE kernels), ADV_EITHER = per launch argument
+// (the dataflow chain with an exploration stage, whose other stages read adv[n]).
+constexpr int ADV_SAMPLE = 0, ADV_TASK = 1, ADV_EITHER = 2;
 __device__ __forceinline__ float kl_coeff_eff(const PolicyArgs& A) {
     return A.kl_coeff_ptr ? A.kl_coeff * __ldcg(A.kl_coeff_ptr) : A.kl_coeff;
 }
@@ -404,8 +412,8 @@ __device__ __forceinline__ void head_setup(const PolicyArgs& A, const float* ls_
 }
 
 // act / old_mean of sample n (task m) and, if `with_ls`, its old log_std (the sample's, or task m's row when the phase stores
-// one row per task), zero above the logical action size dA; returns the sample's advantage.
-template <int DA>
+// one row per task), zero above the logical action size dA; returns the sample's advantage (see ADV_SAMPLE above).
+template <int DA, int ADV = ADV_SAMPLE>
 __device__ __forceinline__ float load_head_sample(const PolicyArgs& A, int64_t n, int m, int dA, bool with_ls, float (&a)[DA],
                                                   float (&mo)[DA], float (&lso)[DA]) {
 #pragma unroll
@@ -417,6 +425,8 @@ __device__ __forceinline__ float load_head_sample(const PolicyArgs& A, int64_t n
         if (with_ls)
             lso[d] = d >= dA ? 0.f : A.ls_per_sample ? __ldg(A.old_ls + n * dA + d) : __ldg(A.old_ls + (int64_t)m * dA + d);
     }
+    if constexpr (ADV == ADV_TASK) return __ldg(A.adv + m);
+    if constexpr (ADV == ADV_EITHER) return A.adv_per_task ? __ldg(A.adv + m) : __ldg(A.adv + n);
     return __ldg(A.adv + n);
 }
 

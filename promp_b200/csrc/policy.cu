@@ -58,7 +58,7 @@ struct GradSmem {
     int last;
 };
 
-template <int DO, int DA, int HID, class Act>
+template <int DO, int DA, int HID, class Act, int ADV = ADV_SAMPLE>
 __device__ __forceinline__ void policy_grad_body(const PolicyArgs& A) {
     using L = PLayout<DO, DA, HID>;
     using C = TileCfg<HID>;
@@ -225,7 +225,7 @@ __device__ __forceinline__ void policy_grad_body(const PolicyArgs& A) {
                 float dmu[DA], dls[DA];
                 if (rb < nb) {
                     float a[DA], mo[DA], lso[DA];
-                    const float adv = load_head_sample<DA>(A, g0 + rb, m, dA, true, a, mo, lso);
+                    const float adv = load_head_sample<DA, ADV>(A, g0 + rb, m, dA, true, a, mo, lso);
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
@@ -315,6 +315,16 @@ template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_kernel(PolicyArgs A) { policy_grad_body<DO, DA, HID, ActTanh>(A); }
 template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_relu_kernel(PolicyArgs A) { policy_grad_body<DO, DA, HID, ActRelu>(A); }
+// PROMP_OBJ_EXPLORE (E-MAML): the same kernel reading the per-task weight adv[m]; separate functions keep the kernels above
+// exactly what they were
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_explore_kernel(PolicyArgs A) {
+    policy_grad_body<DO, DA, HID, ActTanh, ADV_TASK>(A);
+}
+template <int DO, int DA, int HID>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_explore_relu_kernel(PolicyArgs A) {
+    policy_grad_body<DO, DA, HID, ActRelu, ADV_TASK>(A);
+}
 
 // -------------------------------------------------------------------------------------------------
 // Exact Hessian-vector product of the inner surrogate (R-operator: forward-mode tangent through the
@@ -725,6 +735,16 @@ __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, 
     for (int m = 0; m < M; ++m) s += in[(int64_t)m * P + p];
     out[p] = s * scale;
 }
+// out = scale * sum_m a[m] + scale * sum_m b[m]: each sum in the order of reduce_tasks_kernel, so the result equals two
+// promp_reduce_tasks and an add bit for bit
+__global__ void reduce_tasks2_kernel(int M, int P, const float* a, const float* b, float scale, float* out) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= P) return;
+    float sa = 0.f, sb = 0.f;
+    for (int m = 0; m < M; ++m) sa += a[(int64_t)m * P + p];
+    for (int m = 0; m < M; ++m) sb += b[(int64_t)m * P + p];
+    out[p] = __fadd_rn(__fmul_rn(sa, scale), __fmul_rn(sb, scale));
+}
 
 __global__ void adam_tf1_kernel(int P, float* theta, const float* grad, float* mm, float* vv, int32_t* step, float lr,
                                 float b1, float b2, float eps) {
@@ -935,6 +955,12 @@ constexpr bool is_relu() { return std::is_same<Act, ActRelu>::value; }
 
 template <int DO, int DA, int HID, class Act>
 static int launch_grad(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
+    if (A.adv_per_task) {
+        static int occ_x = 0;
+        constexpr auto kx = PROMP_ACT_KERNEL(Act, policy_grad_explore, DO, DA, HID);
+        return launch_policy(kx, (int)sizeof(GradSmem<DO, DA, HID>), occ_x, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
+                             "policy_grad_explore_kernel");
+    }
     static int occ = 0;
     constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_grad, DO, DA, HID);
     return launch_policy(kernel, (int)sizeof(GradSmem<DO, DA, HID>), occ, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
@@ -944,6 +970,16 @@ static int launch_grad(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s
 template <int DO, int DA, int HID, class Act>
 static int launch_grad_any(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
     if constexpr (HID == TC_HID) {
+        if (g_use_tc && A.adv_per_task) {
+            static int occ2 = 0, occ4 = 0;
+            constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_grad_tc_explore, DO, DA, 4);
+            constexpr auto k2 = PROMP_ACT_KERNEL(Act, policy_grad_tc_explore, DO, DA, 2);
+            if (tc_column_groups(DO) == 4)
+                return launch_policy(k4, (int)sizeof(GradTcSmem<DO, DA, 4>), occ4, A,
+                                     PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_explore_kernel", TBT, 512);
+            return launch_policy(k2, (int)sizeof(GradTcSmem<DO, DA, 2>), occ2, A,
+                                 PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_explore_kernel", TBT, 256);
+        }
         if (g_use_tc) {
             static int occ2 = 0, occ4 = 0;
             constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_grad_tc, DO, DA, 4);
@@ -1058,12 +1094,12 @@ static constexpr bool chain_tc_ok() {
     return false;
 }
 
-template <int DO, int DA, int NQ, bool HAS_HVP, class Act>
+template <int DO, int DA, int NQ, bool HAS_HVP, class Act, int ADV = ADV_SAMPLE>
 static int launch_chain_nq(ChainArgs& C, cudaStream_t st) {
     static int configured = 0;
     constexpr int smem = ChainSmem<DO, DA, NQ>::SIZE;
     static_assert(std::is_same<Act, ChainAct>::value, "the chain kernel of this translation unit");
-    constexpr auto kernel = PROMP_CHAIN_KERNEL<DO, DA, NQ, HAS_HVP>;
+    constexpr auto kernel = PROMP_CHAIN_KERNEL<DO, DA, NQ, HAS_HVP, ADV>;
     if (!configured) {
         PROMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         configured = 1;
@@ -1104,8 +1140,11 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
                 C.st[s].counters = (int*)ws + 4 + (CHAIN_MAX_STAGES + s) * M;
                 C.st[s].partial = partial;            // slots are numbered by global item id
             }
-            bool has_hvp = false;
-            for (int s = 0; s < n_stages; ++s) has_hvp = has_hvp || kinds[s] == 1;
+            bool has_hvp = false, has_explore = false;
+            for (int s = 0; s < n_stages; ++s) has_hvp = has_hvp || kinds[s] == 1, has_explore = has_explore || A[s].adv_per_task;
+            if (has_explore)      // one instantiation per shape: HAS_HVP = true runs chains without HVP stages as well
+                return tc_column_groups(DO) == 4 ? launch_chain_nq<DO, DA, 4, true, Act, ADV_EITHER>(C, st)
+                                                 : launch_chain_nq<DO, DA, 2, true, Act, ADV_EITHER>(C, st);
             if (tc_column_groups(DO) == 4)
                 return has_hvp ? launch_chain_nq<DO, DA, 4, true, Act>(C, st) : launch_chain_nq<DO, DA, 4, false, Act>(C, st);
             return has_hvp ? launch_chain_nq<DO, DA, 2, true, Act>(C, st) : launch_chain_nq<DO, DA, 2, false, Act>(C, st);
@@ -1287,6 +1326,13 @@ static int check_policy_args(const char* who, int M, int N, const void* params, 
     return PROMP_OK;
 }
 
+// PROMP_OBJ_EXPLORE is the LOGLIK objective with the per-task weight adv[m]: the kernels see obj_kind LOGLIK and adv_per_task
+static void explore_args(PolicyArgs& A) {
+    if (A.obj_kind != PROMP_OBJ_EXPLORE) return;
+    A.obj_kind = PROMP_OBJ_LOGLIK;
+    A.adv_per_task = 1;
+}
+
 // padded: the bucket instantiations (promp_*_padded entry points), else the exact table
 static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const int32_t* n_valid,
                             const float* params, int64_t param_stride, const float* obs, const float* act,
@@ -1297,7 +1343,7 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
                             void* workspace, int64_t workspace_bytes, void* stream) {
     int st = check_policy_args(n_valid ? "promp_policy_grad_ragged" : "promp_policy_grad", M, N, params, obs, act, adv, old_mean, old_log_std, workspace);
     if (st != PROMP_OK) return st;
-    PROMP_REQUIRE(obj_kind >= 0 && obj_kind <= 3, "promp_policy_grad: bad obj_kind %d", obj_kind);
+    PROMP_REQUIRE(obj_kind >= 0 && obj_kind <= PROMP_OBJ_EXPLORE, "promp_policy_grad: bad obj_kind %d", obj_kind);
     PROMP_REQUIRE(!(out_params && !grad), "promp_policy_grad: out_params needs grad");
     PROMP_REQUIRE((skip_flag == nullptr) == (skip_theta == nullptr) && (unclipped_out == nullptr) == (theta_copy_out == nullptr),
                   "promp_policy_grad_ex: skip_flag / skip_theta and unclipped_out / theta_copy_out come in pairs");
@@ -1311,6 +1357,7 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
     A.grad = grad; A.out_params = out_params; A.sgd_lr = sgd_lr; A.stats = stats; A.n_valid = n_valid;
     A.skip_flag = skip_flag; A.skip_theta = skip_theta; A.unclipped_out = unclipped_out; A.theta_copy_out = theta_copy_out;
     A.obs_dim = obs_dim; A.act_dim = act_dim;
+    explore_args(A);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_grad")
     return (relu_ ? relu_tu::grad : tanh_tu::grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
@@ -1412,9 +1459,15 @@ static int chain_stage_args(const promp_policy_stage* stages, int n_stages, int 
         a.clip_log_std = g.clip_log_std; a.min_log_std = min_log_std; a.stats = g.stats; a.n_valid = g.n_valid;
         a.kl_coeff_ptr = g.kl_coeff_dev;
         if (g.kind == 0) {
-            PROMP_REQUIRE(g.obj_kind >= 0 && g.obj_kind <= 3, "promp_policy_chain: stage %d: bad obj_kind %d", s, g.obj_kind);
+            PROMP_REQUIRE(g.obj_kind >= 0 && g.obj_kind <= PROMP_OBJ_EXPLORE, "promp_policy_chain: stage %d: bad obj_kind %d", s,
+                          g.obj_kind);
             PROMP_REQUIRE(!(g.out_params && !g.grad), "promp_policy_chain: stage %d: out_params needs grad", s);
+            // the exploration stage depends on no other stage and no stage depends on it: the dataflow kernel takes it last
+            PROMP_REQUIRE(g.obj_kind != PROMP_OBJ_EXPLORE || (s == n_stages - 1 && g.param_stride == 0 && !g.out_params),
+                          "promp_policy_chain: stage %d: an EXPLORE stage must be the last stage, at shared parameters "
+                          "(param_stride 0) and without out_params", s);
             a.obj_scale = g.obj_scale; a.clip_eps = g.clip_eps; a.grad = g.grad; a.out_params = g.out_params; a.sgd_lr = g.sgd_lr;
+            explore_args(a);
         } else {
             PROMP_REQUIRE(g.obj_kind == PROMP_OBJ_RATIO || g.obj_kind == PROMP_OBJ_LOGLIK,
                           "promp_policy_chain: stage %d: HVP inner objective must be RATIO or LOGLIK (got %d)", s, g.obj_kind);
@@ -1471,7 +1524,7 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     const int rc = chain_stage_args(stages, n_stages, M, min_log_std, A, kinds, Ns);
     if (rc != PROMP_OK) return rc;
-    PROMP_REQUIRE(!skip_flag || (kinds[0] == 0 && A[0].param_stride == 0),
+    PROMP_REQUIRE(!skip_flag || (kinds[0] == 0 && A[0].param_stride == 0 && !A[0].adv_per_task),
                   "promp_policy_chain: launch re-use is defined for a gradient stage 0 on shared parameters (param_stride 0)");
     for (int k = 0; k < n_stages; ++k) A[k].obs_dim = obs_dim, A[k].act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
@@ -1541,6 +1594,13 @@ extern "C" int promp_reduce_tasks(int M, int P, const float* in, float scale, fl
     PROMP_REQUIRE(M > 0 && P > 0 && in && out, "promp_reduce_tasks: bad arguments");
     reduce_tasks_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(M, P, in, scale, out);
     PROMP_LAUNCH_CHECK("reduce_tasks_kernel");
+    return PROMP_OK;
+}
+
+extern "C" int promp_reduce_tasks2(int M, int P, const float* a, const float* b, float scale, float* out, void* stream) {
+    PROMP_REQUIRE(M > 0 && P > 0 && a && b && out, "promp_reduce_tasks2: bad arguments");
+    reduce_tasks2_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(M, P, a, b, scale, out);
+    PROMP_LAUNCH_CHECK("reduce_tasks2_kernel");
     return PROMP_OK;
 }
 

@@ -314,7 +314,7 @@ __device__ unsigned long long g_phase_clk[16];
 #endif
 // The tile loop of the gradient kernel over the range `sc` describes.  `cached_th` = the parameter vector whose weights
 // the shared-memory tiles currently hold (nullptr: none) - kept across calls by the dataflow kernel.
-template <int DO, int DA, int NQ, class Act, class Sched>
+template <int DO, int DA, int NQ, class Act, class Sched, int ADV = ADV_SAMPLE>
 __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO, DA, NQ>& S, const Sched& sc,
                                               const float*& cached_th) {
     constexpr int HID = TC_HID;
@@ -475,7 +475,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #pragma unroll
             for (int e = 0; e < XR; ++e) S.X[tid + e * TCT] = xq[e];
             if (g + 1 < sc.g_hi) fetch_x(g + 1, xq);
-            if (cq == 0 && r < nb) hadv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, ha, hmo, hlso);
+            if (cq == 0 && r < nb) hadv = load_head_sample<DA, ADV>(A, g0 + r, m, dA, A.ls_per_sample, ha, hmo, hlso);
         } else {
             for (int i = tid; i < TBT * DOP; i += TCT) {
                 const int b = i / DOP, c = i % DOP;
@@ -555,7 +555,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     for (int d = 0; d < DA; ++d) a[d] = ha[d], mo[d] = hmo[d], lso[d] = hlso[d];
                     adv = hadv;
                 } else {
-                    adv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
+                    adv = load_head_sample<DA, ADV>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
                 }
                 HeadOut<DA> o;
                 if (A.ls_per_sample) {
@@ -670,7 +670,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
 #endif
 }
 
-template <int DO, int DA, int NQ, class Act>
+template <int DO, int DA, int NQ, class Act, int ADV = ADV_SAMPLE>
 __device__ __forceinline__ void policy_grad_tc_body(const PolicyArgs& A) {
     using SM = GradTcSmem<DO, DA, NQ>;
     using L = PLayout<DO, DA, TC_HID>;
@@ -680,13 +680,22 @@ __device__ __forceinline__ void policy_grad_tc_body(const PolicyArgs& A) {
     reuse_produce<L::P, L::LS, DA>(A);
     const UniformSched sc(A.M, A.N, A.q, A.kmax, TBT);
     const float* cached_th = nullptr;
-    grad_tc_tiles<DO, DA, NQ, Act>(A, S, sc, cached_th);
+    grad_tc_tiles<DO, DA, NQ, Act, UniformSched, ADV>(A, S, sc, cached_th);
 }
 // one kernel per activation, as in policy.cu: *_kernel = tanh, *_relu_kernel = ReLU
 template <int DO, int DA, int NQ>
 __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_kernel(PolicyArgs A) { policy_grad_tc_body<DO, DA, NQ, ActTanh>(A); }
 template <int DO, int DA, int NQ>
 __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_relu_kernel(PolicyArgs A) { policy_grad_tc_body<DO, DA, NQ, ActRelu>(A); }
+// PROMP_OBJ_EXPLORE: per-task weight adv[m] (see policy_grad_explore_kernel)
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_explore_kernel(PolicyArgs A) {
+    policy_grad_tc_body<DO, DA, NQ, ActTanh, ADV_TASK>(A);
+}
+template <int DO, int DA, int NQ>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_explore_relu_kernel(PolicyArgs A) {
+    policy_grad_tc_body<DO, DA, NQ, ActRelu, ADV_TASK>(A);
+}
 
 
 // =================================================================================================================
@@ -1197,7 +1206,9 @@ using ChainAct = ActRelu;
 #define PROMP_CHAIN_KERNEL policy_chain_tc_kernel
 using ChainAct = ActTanh;
 #endif
-template <int DO, int DA, int NQ, bool HAS_HVP = true>
+// ADV = ADV_EITHER: the chain has an exploration stage (PROMP_OBJ_EXPLORE, the last stage): its items read the per-task weight
+// adv[m] and wait for no other stage.
+template <int DO, int DA, int NQ, bool HAS_HVP = true, int ADV = ADV_SAMPLE>
 __global__ void __launch_bounds__(128 * NQ, 1) PROMP_CHAIN_KERNEL(const __grid_constant__ ChainArgs C) {
     using Act = ChainAct;
     using GS = GradTcSmem<DO, DA, NQ>;
@@ -1243,11 +1254,13 @@ __global__ void __launch_bounds__(128 * NQ, 1) PROMP_CHAIN_KERNEL(const __grid_c
         sc.first_item = I.item_base + I.reg_item0[r] + mr * per_task;
         sc.n_items = per_task;
         sc.ready_prev = (s > 0 && !(s == 1 && skip0)) ? C.ready + (s - 1) * C.M : nullptr;
+        if constexpr (ADV == ADV_EITHER)
+            if (C.st[s].adv_per_task) sc.ready_prev = nullptr;
         sc.ready_mine = C.ready + s * C.M;
         CCLK(0);
         if (!HAS_HVP || I.kind == 0) {
             cached_h = nullptr;
-            grad_tc_tiles<DO, DA, NQ, Act>(C.st[s], G, sc, cached_g);
+            grad_tc_tiles<DO, DA, NQ, Act, ItemSched, ADV>(C.st[s], G, sc, cached_g);
         } else if constexpr (HAS_HVP) {
             cached_g = nullptr;
             hvp_tc_tiles<DO, DA, NQ, Act>(C.st[s], H, sc, cached_h);

@@ -632,6 +632,39 @@ __global__ void adj_avg_rewards_kernel(int64_t n, const float* rew, double mean,
     if (i < n) out[i] = (float)(((double)rew[i] - mean) * inv);
 }
 
+// E-MAML coefficient c_m = (mean_m r - mean_all) / (std_all + 1e-8) from the per-task reward sums stats[m][5..6]
+// (samplers/meta_sample_processor.py:40-44 averaged over task m; trpo_maml.py:137-144).  n_m = n_valid[m] or N.  One warp;
+// lane 0 sums the totals in task order in float64.  totals_out (may be NULL): [sum r, sum r^2, sum n] of these tasks.
+// coeff (may be NULL): c_m, from totals_in when given (the totals of every rank), else from this launch's totals.  Every
+// operation is rounded on its own (no contraction), in the order of the eager torch expression it replaces.
+__global__ void emaml_coeff_kernel(int M, const double* __restrict__ stats, const int32_t* __restrict__ n_valid, int N,
+                                   const double* __restrict__ totals_in, double* __restrict__ totals_out, float* __restrict__ coeff) {
+    __shared__ double tot[3];
+    const int lane = threadIdx.x;
+    if (lane == 0) {
+        double s = 0.0, q = 0.0, n = 0.0;
+        for (int m = 0; m < M; ++m) {
+            s = __dadd_rn(s, stats[(int64_t)m * 8 + 5]);
+            q = __dadd_rn(q, stats[(int64_t)m * 8 + 6]);
+            n = __dadd_rn(n, (double)(n_valid ? n_valid[m] : N));
+        }
+        if (totals_out) totals_out[0] = s, totals_out[1] = q, totals_out[2] = n;
+        tot[0] = totals_in ? totals_in[0] : s;
+        tot[1] = totals_in ? totals_in[1] : q;
+        tot[2] = totals_in ? totals_in[2] : n;
+    }
+    __syncwarp();
+    if (!coeff) return;
+    const double mean = __ddiv_rn(tot[0], tot[2]);
+    const double var = fmax(__dsub_rn(__ddiv_rn(tot[1], tot[2]), __dmul_rn(mean, mean)), 0.0);
+    const double den = __dadd_rn(__dsqrt_rn(var), 1e-8);
+    for (int m = lane; m < M; m += 32) {
+        const int nm = n_valid ? n_valid[m] : N;
+        coeff[m] = nm > 0 ? __double2float_rn(__ddiv_rn(__dsub_rn(__ddiv_rn(stats[(int64_t)m * 8 + 5], (double)nm), mean), den))
+                          : 0.f;
+    }
+}
+
 // LinearFeatureBaseline.predict (baselines/linear_baseline.py:17-33) for a flat list of paths
 __global__ void baseline_predict_kernel(int n_paths, const int32_t* __restrict__ path_off, int Do, const float* __restrict__ obs,
                                         const double* __restrict__ coeffs, double* __restrict__ out) {
@@ -815,6 +848,27 @@ extern "C" int promp_adj_avg_rewards(int64_t n, const float* rew, double mean, d
                                                                                          1.0 / (std + 1e-8), out);
     PROMP_LAUNCH_CHECK("adj_avg_rewards_kernel");
     return PROMP_OK;
+}
+
+static int emaml_launch(const char* who, int M, const double* stats, const int32_t* n_valid, int N, const double* totals_in,
+                        double* totals_out, float* coeff, void* stream) {
+    PROMP_REQUIRE(M > 0 && stats && (n_valid || N > 0), "%s: bad arguments (M = %d, N = %d)", who, M, N);
+    emaml_coeff_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(M, stats, n_valid, N, totals_in, totals_out, coeff);
+    PROMP_LAUNCH_CHECK("emaml_coeff_kernel");
+    return PROMP_OK;
+}
+extern "C" int promp_emaml_coeff(int M, const double* stats, const int32_t* n_valid, int N, float* coeff, void* stream) {
+    PROMP_REQUIRE(coeff, "promp_emaml_coeff: null coeff");
+    return emaml_launch("promp_emaml_coeff", M, stats, n_valid, N, nullptr, nullptr, coeff, stream);
+}
+extern "C" int promp_emaml_totals(int M, const double* stats, const int32_t* n_valid, int N, double* totals, void* stream) {
+    PROMP_REQUIRE(totals, "promp_emaml_totals: null totals");
+    return emaml_launch("promp_emaml_totals", M, stats, n_valid, N, nullptr, totals, nullptr, stream);
+}
+extern "C" int promp_emaml_finish(int M, const double* stats, const int32_t* n_valid, int N, const double* totals, float* coeff,
+                                  void* stream) {
+    PROMP_REQUIRE(totals && coeff, "promp_emaml_finish: null totals / coeff");
+    return emaml_launch("promp_emaml_finish", M, stats, n_valid, N, totals, nullptr, coeff, stream);
 }
 
 // ---- variable-length paths: same kernel driven by a per-task path table ------------------------------------------

@@ -28,6 +28,8 @@ class MAMLAlgo(object):
         trainable_inner_step_size (must be False, as in every shipped reference config)
     """
     inner_obj_kind = _lib.OBJ_RATIO
+    CHAIN_MAX_STAGES = 6          # promp_policy_chain's stage limit
+    STATS_SLOTS = 16              # per-evaluation stats buffers kept per (S, M), see _stats_rows
 
     def __init__(self, policy, inner_lr=0.1, meta_batch_size=20, num_inner_grad_steps=1,
                  trainable_inner_step_size=False):
@@ -45,6 +47,7 @@ class MAMLAlgo(object):
         self._optimization_keys = None
         self._ws = None
         self._ws_chain = None
+        self._stats_ring = {}
         # the gradient chain of a meta-objective evaluation as ONE dataflow launch (promp_policy_chain) or as one launch per stage
         self.use_chain = os.environ.get('PROMP_B200_CHAIN', '1') != '0'
 
@@ -56,6 +59,21 @@ class MAMLAlgo(object):
         if self._ws is None or self._ws.numel() * 4 < need:
             self._ws = torch.zeros((need + 3) // 4, dtype=torch.int32, device=p.device)   # counters start at zero
         return self._ws
+
+    def _stats_rows(self, S):
+        """The [S, M, 4] float32 stats buffer of one evaluation (row s = launch s), taken in turn from STATS_SLOTS buffers
+        that are allocated and zero-filled together on first use, like the workspaces.  The kernels write columns 0-2 and
+        never column 3, which therefore stays zero: an evaluation's stats are defined in full without a fill per evaluation
+        (a captured iteration replays no fill).  A buffer is handed out again STATS_SLOTS evaluations later; every consumer
+        reads its rows on the stream before that (promp_meta_loss_terms, the loss-term sums, the tests' clones)."""
+        import torch
+        M = self.meta_batch_size
+        ring = self._stats_ring.get(S)
+        if ring is None:
+            ring = self._stats_ring[S] = [torch.zeros(self.STATS_SLOTS, S, M, 4, dtype=torch.float32, device=self.policy.device), 0]
+        buf = ring[0][ring[1]]
+        ring[1] = (ring[1] + 1) % self.STATS_SLOTS
+        return buf
 
     def _phase_of(self, samples):
         """samples: list (len M) of per-task dicts -> PhaseData on the device."""
@@ -86,9 +104,10 @@ class MAMLAlgo(object):
         return phase
 
     def _grad(self, phase, params, stride, obj_kind, obj_scale=1.0, clip_eps=0.0, kl_coeff=0.0, clip_log_std=0,
-              grad=None, out_params=None, sgd_lr=0.0, stats=None, produce=None, reuse=None):
+              grad=None, out_params=None, sgd_lr=0.0, stats=None, produce=None, reuse=None, adv=None):
         """One promp_policy_grad launch.  produce / reuse = (flag int32[1], theta copy [P]): the launch re-use protocol of
-        promp_policy_grad_ex (the _adapt launch produces, the identical inner pass of the first Adam epoch re-uses)."""
+        promp_policy_grad_ex (the _adapt launch produces, the identical inner pass of the first Adam epoch re-uses).
+        adv: the weights in place of phase.adv (OBJ_EXPLORE: the per-task E-MAML coefficient [M])."""
         p = self.policy
         ws = self._workspace(phase.N)
         full = getattr(phase, 'log_std_full', None)
@@ -97,21 +116,22 @@ class MAMLAlgo(object):
         skip = (_lib.ptr(reuse[0]), _lib.ptr(reuse[1])) if reuse is not None else (None, None)
         prod = (_lib.ptr(produce[0]), _lib.ptr(produce[1])) if produce is not None else (None, None)
         _lib.call(p.entries['grad_ex'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, phase.N, _lib.ptr(n_valid),
-                  _lib.ptr(params), stride, _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.adv),
+                  _lib.ptr(params), stride, _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.adv if adv is None else adv),
                   _lib.ptr(phase.mean), _lib.ptr(old_ls), per_sample, obj_kind, float(obj_scale), float(clip_eps),
                   float(kl_coeff), int(clip_log_std), float(p.min_log_std), _lib.ptr(grad), _lib.ptr(out_params),
                   float(sgd_lr), _lib.ptr(stats), skip[0], skip[1], prod[0], prod[1], _lib.ptr(ws), ws.numel() * 4, _lib.stream())
 
     def _stage(self, kind, phase, params, stride, obj_kind, obj_scale=1.0, clip_eps=0.0, kl_coeff=0.0, clip_log_std=0, grad=None,
-               out_params=None, sgd_lr=0.0, vec=None, out=None, stats=None, kl_coeff_dev=None):
+               out_params=None, sgd_lr=0.0, vec=None, out=None, stats=None, kl_coeff_dev=None, adv=None):
         """One promp_policy_stage (kind 0: the arguments of _grad, kind 1: those of _hvp)."""
         full = getattr(phase, 'log_std_full', None)
         old_ls, per_sample = (full, 1) if full is not None else (phase.log_std, 0)
         st = _lib.PolicyStage()
         st.kind, st.N, st.n_valid = kind, phase.N, _lib.ptr(getattr(phase, 'n_valid', None))
         st.params, st.param_stride = _lib.ptr(params), stride
-        st.obs, st.act, st.adv, st.old_mean, st.old_log_std = (_lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.adv),
-                                                               _lib.ptr(phase.mean), _lib.ptr(old_ls))
+        st.obs, st.act, st.adv, st.old_mean, st.old_log_std = (_lib.ptr(phase.obs), _lib.ptr(phase.act),
+                                                               _lib.ptr(phase.adv if adv is None else adv), _lib.ptr(phase.mean),
+                                                               _lib.ptr(old_ls))
         st.ls_per_sample, st.obj_kind, st.obj_scale, st.clip_eps = per_sample, obj_kind, float(obj_scale), float(clip_eps)
         st.kl_coeff, st.clip_log_std = float(kl_coeff), int(clip_log_std)
         st.grad, st.out_params, st.sgd_lr = _lib.ptr(grad), _lib.ptr(out_params), float(sgd_lr)
@@ -165,7 +185,7 @@ class MAMLAlgo(object):
             if getattr(self, '_reuse_bufs', None) is None:
                 self._reuse_bufs = (torch.zeros(1, dtype=torch.int32, device=p.device),
                                     torch.empty(P, dtype=torch.float32, device=p.device))
-            stats_all = torch.empty(self.num_inner_grad_steps + 1, M, 4, dtype=torch.float32, device=p.device)
+            stats_all = self._stats_rows(self.num_inner_grad_steps + 1)
             produce, stats = self._reuse_bufs, stats_all[0]
             self._adapt_cache = dict(phase=phase, adv=phase.adv, gen=getattr(phase, 'generation', 0), grad=grad, new=new,
                                      stats_all=stats_all)
@@ -187,21 +207,37 @@ class MAMLAlgo(object):
 
     # ------------------------------------------------------------------------------------ meta objective
     def _meta_pass(self, theta, phases, outer_obj_kind, clip_eps, inner_kl_coeffs, want_grad, outer_kl_coeff=0.0,
-                   outer_obj_scale=1.0, reduce=True, inner_kl_coeffs_dev=None):
+                   outer_obj_scale=1.0, reduce=True, inner_kl_coeffs_dev=None, explore=None):
         """One evaluation of the meta objective (and optionally its gradient) at `theta` [P].
 
         Returns dict(grad=[P] or None (local sum over tasks / M_global, NOT yet all-reduced),
                      surr=[M] outer surrogate per task, outer_kl=[M], inner_kl=[S-1, M]).
         reduce=False leaves the per-task gradients in out['grad_tasks'] [M, P] for the fused reduce + all-reduce + Adam
-        kernel (promp_meta_update) and skips promp_reduce_tasks."""
+        kernel (promp_meta_update) and skips promp_reduce_tasks.
+        explore: the E-MAML coefficient c [M] (device) or None.  The exploration term -c_m * mean logp_theta(a|x) on the
+        phase-0 data (trpo_maml.py:137-144) is then one more gradient stage (OBJ_EXPLORE at theta, clipped log_std) of the
+        chain; out['explore'] = its value per task [M], and its gradient is summed into out['grad'] by the same reduction."""
         import torch
         p = self.policy
         M, P, S = self.meta_batch_size, p.num_params, len(phases)
         dev = p.device
+        assert explore is None or reduce, "the exploration gradient is added by promp_reduce_tasks2 (reduce=True)"
+        x_stats = torch.empty(M, 4, dtype=torch.float32, device=dev) if explore is not None else None
+        x_grad = torch.empty(M, P, dtype=torch.float32, device=dev) if explore is not None and want_grad else None
+
+        def reduced(v):
+            flat = torch.empty(P, dtype=torch.float32, device=dev)
+            if x_grad is None:
+                _lib.call('promp_reduce_tasks', M, P, _lib.ptr(v), 1.0 / (M * world_size()), _lib.ptr(flat), _lib.stream())
+            else:
+                _lib.call('promp_reduce_tasks2', M, P, _lib.ptr(v), _lib.ptr(x_grad), 1.0 / (M * world_size()), _lib.ptr(flat),
+                          _lib.stream())
+            return flat
+
+        def explore_launch():
+            self._grad(phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=x_grad, stats=x_stats, adv=explore)
         cur, stride, clip = theta, 0, 1              # step 0 = distribution_info_sym(params=None): clipped log_std
         chain = []
-        # one stats buffer per evaluation, fully written by the kernels (no fills, no copies): row s = launch s
-        stats_all = torch.empty(S, M, 4, dtype=torch.float32, device=dev)
         # The inner pass at step 0 repeats the _adapt launch as long as theta has not been updated since (first Adam epoch,
         # "loss before" passes): aim it at the SAME output buffers and let the kernel skip itself after verifying on the
         # device that the parameters are bit-identical and the step-0 log_std clip is inactive.  Host-side conditions: same
@@ -214,6 +250,8 @@ class MAMLAlgo(object):
         if reuse0:
             stats_all = cache['stats_all']
             self._adapt_cache = None          # one consumer: later passes (updated theta) use their own buffers
+        else:
+            stats_all = self._stats_rows(S)   # one stats buffer per evaluation (no fills, no copies): row s = launch s
         if inner_kl_coeffs_dev is not None and not self.use_chain:
             # the stand-alone entry points take the coefficient by value: read the device vector back (eager diagnostics only)
             host = inner_kl_coeffs_dev.cpu().numpy()
@@ -245,14 +283,21 @@ class MAMLAlgo(object):
                                               kl_coeff_dev=None if inner_kl_coeffs_dev is None else inner_kl_coeffs_dev[s:s + 1]))
                     chain.append(v)       # the stage list holds raw pointers: keep every buffer alive until the launch is enqueued
                     v = v_out
+            x_separate = explore is not None and len(stages) >= self.CHAIN_MAX_STAGES
+            if explore is not None and not x_separate:
+                # last stage, waits for no other: in the dataflow kernel it fills the tail of the backward chain
+                stages.append(self._stage(0, phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=x_grad, stats=x_stats,
+                                          adv=explore))
             self._run_chain(stages, reuse=self._reuse_bufs if reuse0 else None)
+            if x_separate:
+                explore_launch()
             out = dict(surr=stats_all[S - 1, :, 0], outer_kl=stats_all[S - 1, :, 1], inner_kl=stats_all[:S - 1, :, 1],
                        stats_all=stats_all, grad=None)
+            if x_stats is not None:
+                out['explore'] = x_stats[:, 0]
             if want_grad:
                 if reduce:
-                    flat = torch.empty(P, dtype=torch.float32, device=dev)
-                    _lib.call('promp_reduce_tasks', M, P, _lib.ptr(v), 1.0 / (M * world_size()), _lib.ptr(flat), _lib.stream())
-                    out['grad'] = flat
+                    out['grad'] = reduced(v)
                 else:
                     out['grad_tasks'] = v
             return out
@@ -281,10 +326,12 @@ class MAMLAlgo(object):
                 v_out = torch.empty(M, P, dtype=torch.float32, device=dev)
                 self._hvp(phases[s], prm, strd, v, v_out, inner_kl_coeffs[s], clp)
                 v = v_out
+        if explore is not None:
+            explore_launch()
+            out['explore'] = x_stats[:, 0]
+        if want_grad:
             if reduce:
-                flat = torch.empty(P, dtype=torch.float32, device=dev)
-                _lib.call('promp_reduce_tasks', M, P, _lib.ptr(v), 1.0 / (M * world_size()), _lib.ptr(flat), _lib.stream())
-                out['grad'] = flat
+                out['grad'] = reduced(v)
             else:
                 out['grad_tasks'] = v
         return out

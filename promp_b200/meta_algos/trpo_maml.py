@@ -29,11 +29,12 @@ class TRPOMAML(MAMLAlgo):
     # ---- E-MAML exploration term (:137-144): surr_i += -mean(adj_avg_rewards_i) * mean(logp_theta(a0 | x0))
     def _exploration_coeff(self, phases):
         """c_i = mean_n adj_avg_rewards_i of the LAST phase = (mean r_i - mean r_all) / (std r_all + 1e-8), on the
-        device from the processing kernel's per-task sums (global over ranks)."""
+        device from the processing kernel's per-task sums (global over ranks), expanded to [M, N].  The eager statement of
+        exploration_coeff_dev for fixed-horizon phases, kept as its reference; the algorithms no longer call it."""
         import torch
         last = phases[-1]
         if getattr(last, 'n_valid', None) is not None or getattr(phases[0], 'n_valid', None) is not None:
-            raise NotImplementedError("promp_b200: the E-MAML exploration term is implemented for fixed-horizon paths only")
+            raise NotImplementedError("_exploration_coeff covers fixed-horizon paths; exploration_coeff_dev covers both")
         if getattr(last, 'adj_avg_rewards_mean', None) is not None:
             # reference-style sample dicts (MAMLAlgo._phase_of): the caller's processor already computed adj_avg_rewards
             return last.adj_avg_rewards_mean.view(-1, 1).expand(last.M, phases[0].N).contiguous()
@@ -50,21 +51,48 @@ class TRPOMAML(MAMLAlgo):
             last._explore_adv = c.view(-1, 1).expand(last.M, phases[0].N).contiguous()
         return last._explore_adv
 
+    def exploration_coeff_dev(self, phases):
+        """c [M] float32 on the device: the task means of adj_avg_rewards of the LAST phase, over each task's valid samples
+        (promp_emaml_coeff on the processing kernel's per-task reward sums; totals summed over ranks).  No host arithmetic
+        and no host copies: a CUDA graph records it.  Computed once per phase and data generation."""
+        import torch
+        last = phases[-1]
+        if getattr(last, 'adj_avg_rewards_mean', None) is not None:
+            return last.adj_avg_rewards_mean          # reference-style sample dicts: already the task means
+        if getattr(last, 'stats', None) is None:
+            raise NotImplementedError("exploration=True needs 'adj_avg_rewards' in the sample dicts or a phase processed by "
+                                      "promp_b200's MetaSampleProcessor")
+        gen = getattr(last, 'generation', 0)
+        cached = getattr(last, '_emaml_coeff', None)
+        if cached is not None and cached[0] == gen:
+            return cached[1]
+        M, dev = last.M, last.stats.device
+        n_valid = getattr(last, 'n_valid', None)
+        c = torch.empty(M, dtype=torch.float32, device=dev)
+        if world_size() > 1:
+            tot = torch.empty(3, dtype=torch.float64, device=dev)
+            _lib.call('promp_emaml_totals', M, _lib.ptr(last.stats), _lib.ptr(n_valid), last.N, _lib.ptr(tot), _lib.stream())
+            allreduce_sum_(tot)
+            _lib.call('promp_emaml_finish', M, _lib.ptr(last.stats), _lib.ptr(n_valid), last.N, _lib.ptr(tot), _lib.ptr(c),
+                      _lib.stream())
+        else:
+            _lib.call('promp_emaml_coeff', M, _lib.ptr(last.stats), _lib.ptr(n_valid), last.N, _lib.ptr(c), _lib.stream())
+        last._emaml_coeff = (gen, c)
+        return c
+
     def _exploration_term(self, theta, phases, want_grad):
-        """(-c_i * mean logp) per task [M] and, optionally, its gradient w.r.t. theta per task [M,P]: the LOGLIK
-        objective of promp_policy_grad on the phase-0 data with the constant c_i in place of the advantages."""
+        """(-c_i * mean logp) per task [M] and, optionally, its gradient w.r.t. theta per task [M,P]: one OBJ_EXPLORE
+        launch of promp_policy_grad on the phase-0 data.  The meta-objective passes run the same stage inside their chain
+        (MAMLAlgo._meta_pass(explore=...)); this stand-alone form serves diagnostics and tests."""
         import torch
         p = self.policy
-        ph0 = phases[0]
-        adv_saved = ph0.adv
-        ph0.adv = self._exploration_coeff(phases)
-        st = torch.zeros(self.meta_batch_size, 4, dtype=torch.float32, device=p.device)
+        st = torch.empty(self.meta_batch_size, 4, dtype=torch.float32, device=p.device)
         g = torch.empty(self.meta_batch_size, p.num_params, dtype=torch.float32, device=p.device) if want_grad else None
-        try:
-            self._grad(ph0, theta, 0, _lib.OBJ_LOGLIK, clip_log_std=1, grad=g, stats=st)
-        finally:
-            ph0.adv = adv_saved
+        self._grad(phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=g, stats=st, adv=self.exploration_coeff_dev(phases))
         return st[:, 0], g
+
+    def _explore(self, phases):
+        return self.exploration_coeff_dev(phases) if self.exploration else None
 
     # meta objective = mean_i -mean(ratio*adv) (:135,152); constraint = mean_i mean KL(old || theta_i') (:133,149)
     def loss_terms_dev(self, theta, phases, out=None):
@@ -72,13 +100,13 @@ class TRPOMAML(MAMLAlgo):
         into `out` when given.  No host interaction."""
         import torch
         S1 = self.num_inner_grad_steps
-        res = self._meta_pass(theta, phases, _lib.OBJ_RATIO, 0.0, [0.0] * S1, want_grad=False)
+        res = self._meta_pass(theta, phases, _lib.OBJ_RATIO, 0.0, [0.0] * S1, want_grad=False, explore=self._explore(phases))
         if out is None:
             out = torch.empty(S1 + 2, dtype=torch.float32, device=self.policy.device)
         _lib.call('promp_meta_loss_terms', S1 + 1, self.meta_batch_size, _lib.ptr(res['stats_all']),
                   1.0 / (self.meta_batch_size * world_size()), None, S1 + 2, _lib.ptr(out), _lib.stream())
         if self.exploration:
-            out[0] += self._exploration_term(theta, phases, False)[0].sum() / (self.meta_batch_size * world_size())
+            out[0] += res['explore'].sum() / (self.meta_batch_size * world_size())
         allreduce_sum_(out)
         return out
 
@@ -87,14 +115,7 @@ class TRPOMAML(MAMLAlgo):
         ranks, on the device."""
         zeros = [0.0] * self.num_inner_grad_steps
         if which == 'loss':
-            res = self._meta_pass(theta, phases, _lib.OBJ_RATIO, 0.0, zeros, want_grad=True)
-            if self.exploration:
-                import torch
-                _, g = self._exploration_term(theta, phases, True)
-                extra = torch.empty_like(res['grad'])
-                _lib.call('promp_reduce_tasks', self.meta_batch_size, self.policy.num_params, _lib.ptr(g),
-                          1.0 / (self.meta_batch_size * world_size()), _lib.ptr(extra), _lib.stream())
-                res['grad'] += extra
+            res = self._meta_pass(theta, phases, _lib.OBJ_RATIO, 0.0, zeros, want_grad=True, explore=self._explore(phases))
         else:
             res = self._meta_pass(theta, phases, _lib.OBJ_NONE, 0.0, zeros, want_grad=True, outer_kl_coeff=1.0)
         allreduce_sum_(res['grad'])
@@ -112,10 +133,11 @@ class TRPOMAML(MAMLAlgo):
 
     @property
     def graph_capturable(self):
-        # the E-MAML coefficient is assembled with host scalars.  (Round 2 ran several ranks eagerly because the ~250-launch
-        # capture was invalidated now and then: that was Python's cyclic GC destroying an older CUDAGraph during the capture,
-        # fixed in Trainer.capture_graph.)
-        return not self.exploration
+        # Every iteration is device-only, E-MAML included: its coefficient is promp_emaml_coeff (plus an NCCL all-reduce of
+        # three float64 totals with several ranks).  The Trainer still runs early-terminating envs eagerly.  (Round 2 ran
+        # several ranks eagerly because the ~250-launch capture was invalidated now and then: that was Python's cyclic GC
+        # destroying an older CUDAGraph during the capture, fixed in Trainer.capture_graph.)
+        return True
 
     def optimize_phases(self, phases, out=None, want_terms=True):
         """optimize_policy on PhaseData objects up to the verdict on the first line-search group, everything left on the

@@ -28,22 +28,18 @@ class VPGMAML(MAMLAlgo):
         self.inner_obj_kind = _lib.OBJ_RATIO if inner_type == 'likelihood_ratio' else _lib.OBJ_LOGLIK
         self.optimizer.build(self.policy)
 
-    # the E-MAML term is shared with TRPOMAML (same formula, vpg_maml.py:137-144 == trpo_maml.py:137-144)
+    # the E-MAML term is shared with TRPOMAML (same formula, vpg_maml.py:137-144 == trpo_maml.py:137-144).  The Trainer never
+    # captures VPGMAML into a CUDA graph (it has no optimize_phases); its coefficient is device-side all the same.
     _exploration_coeff = TRPOMAML._exploration_coeff
+    exploration_coeff_dev = TRPOMAML.exploration_coeff_dev
     _exploration_term = TRPOMAML._exploration_term
+    _explore = TRPOMAML._explore
 
     def _objective_pass(self, phases, want_grad):
-        import torch
         zeros = [0.0] * self.num_inner_grad_steps
-        res = self._meta_pass(self.policy.theta, phases, _lib.OBJ_LOGLIK, 0.0, zeros, want_grad)
+        res = self._meta_pass(self.policy.theta, phases, _lib.OBJ_LOGLIK, 0.0, zeros, want_grad, explore=self._explore(phases))
         if self.exploration:
-            val, g = self._exploration_term(self.policy.theta, phases, want_grad)
-            res['surr'] = res['surr'] + val
-            if want_grad:
-                extra = torch.empty_like(res['grad'])
-                _lib.call('promp_reduce_tasks', self.meta_batch_size, self.policy.num_params, _lib.ptr(g),
-                          1.0 / (self.meta_batch_size * world_size()), _lib.ptr(extra), _lib.stream())
-                res['grad'] += extra
+            res['surr'] = res['surr'] + res['explore']
         return res
 
     def loss_terms(self, res):
