@@ -66,8 +66,10 @@ enum {
  * promp_num_params, promp_policy_layout and the workspace sizes do not depend on the activation. */
 #define PROMP_HIDDEN_WIDTH_MASK 0xFF
 #define PROMP_ACT_RELU 0x100
-/* baseline kinds of promp_process_samples */
-enum { PROMP_BASELINE_ZERO = 0, PROMP_BASELINE_LINEAR_FEATURE = 1 };
+/* baseline kinds of promp_process_samples.  LINEAR_TIME (baselines/linear_baseline.py:109-126) fits [t, t^2, t^3, 1],
+ * t = step / 100, and never reads obs; its coefficients are [M,4].  GIVEN: the caller supplies the per-sample baseline
+ * values (promp_process_samples_given); no fit, no coefficients. */
+enum { PROMP_BASELINE_ZERO = 0, PROMP_BASELINE_LINEAR_FEATURE = 1, PROMP_BASELINE_LINEAR_TIME = 2, PROMP_BASELINE_GIVEN = 3 };
 
 const char* promp_last_error(void);
 int promp_version(void);
@@ -229,9 +231,11 @@ int promp_paths_finalize_ex(int M, int E, int timeline_len, int max_paths, int m
  * matrix, solve, scans and moments run in float64 like the reference's numpy.
  *
  *   obs [M,E,H,Do]  rew [M,E,H]
+ *   baseline_kind: PROMP_BASELINE_ZERO, _LINEAR_FEATURE or _LINEAR_TIME (LinearTimeBaseline, linear_baseline.py:109-126:
+ *           the same fit and predict over the features [t, t^2, t^3, 1]; obs is not read)
  * outputs:
  *   returns [M,E,H]  adv [M,E,H]
- *   coeffs  [M,F] float64, F = 2*Do+4 (may be NULL)
+ *   coeffs  [M,F] float64, F = 2*Do+4 (LINEAR_FEATURE) or 4 (LINEAR_TIME) (may be NULL)
  *   stats   [M,8] float64: sum R_0, sum G, sum G^2, max G, min G (G = undiscounted return per path),
  *           sum r, sum r^2, reg_coeff finally used            (may be NULL)
  *   workspace: scratch, >= promp_process_workspace_bytes(M,E,H,Do) bytes.  It must be ZERO-FILLED before its first
@@ -264,6 +268,24 @@ int promp_process_samples_ragged(int M, int max_paths, int max_samples, int obs_
                                  void* workspace, int64_t workspace_bytes, void* stream);
 
 /*
+ * Any baseline object (samplers/base.py:99-108 accepts whatever has fit / predict): the caller fitted it and evaluated
+ * predict(path) itself; the kernel takes those values and runs everything downstream of the reference's predict exactly
+ * as above (discounted returns, GAE, normalisation / positive shift, stats).  PROMP_BASELINE_GIVEN.
+ *   baseline_values [M,NS] float64 device memory in the phase's sample layout (NS = E*H, or max_samples on the ragged
+ *   layout, where positions past path_off[m][n_paths[m]] are not read).  No coefficients are written; stats[m][7] = 0.
+ *   The workspace is the one of promp_process_workspace_bytes / _ragged for the same shape.
+ */
+int promp_process_samples_given(int M, int E, int H, int obs_dim, const float* obs, const float* rew,
+                                const double* baseline_values, double discount, double gae_lambda, int normalize_adv,
+                                int positive_adv, float* returns, float* adv, double* stats,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+int promp_process_samples_ragged_given(int M, int max_paths, int max_samples, int obs_dim, const float* obs, const float* rew,
+                                       const int32_t* path_off, const int32_t* n_paths, const double* baseline_values,
+                                       double discount, double gae_lambda, int normalize_adv, int positive_adv,
+                                       float* returns, float* adv, double* stats,
+                                       void* workspace, int64_t workspace_bytes, void* stream);
+
+/*
  * Launch geometry of the processing kernel for one shape, computed on the host (no CUDA call).  It replaces no reference
  * function: it exists so that tests can name the code path a shape exercises.  Fixed horizon (ragged = 0): max_paths = E,
  * NS = E*H, as in promp_process_samples.  Variable-length paths (ragged = 1): max_paths and NS = max_samples as in
@@ -289,6 +311,17 @@ int promp_baseline_fit(int n_paths, int n_samples, int obs_dim, const float* obs
                        void* workspace, int64_t workspace_bytes, void* stream);
 int promp_baseline_predict(int n_paths, int n_samples, int obs_dim, const float* obs, const int32_t* path_off,
                            const double* coeffs, double* out, void* stream);
+/*
+ * The same fit / predict for either linear baseline (baselines/linear_baseline.py:55-77, 17-33): kind =
+ * PROMP_BASELINE_LINEAR_FEATURE (features :101-106, exactly promp_baseline_fit / _predict) or PROMP_BASELINE_LINEAR_TIME
+ * (LinearTimeBaseline, features :122-126: [t, t^2, t^3, 1], coeffs [4]; obs is not read and may be NULL).  The workspace
+ * is sized by promp_baseline_fit_workspace_bytes for both kinds.
+ */
+int promp_baseline_fit_ex(int kind, int n_paths, int n_samples, int obs_dim, const float* obs, const double* target,
+                          const int32_t* path_off, double reg_coeff, double* coeffs, double* reg_used,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+int promp_baseline_predict_ex(int kind, int n_paths, int n_samples, int obs_dim, const float* obs, const int32_t* path_off,
+                              const double* coeffs, double* out, void* stream);
 
 /*
  * Fused outer update of one Adam epoch (optimizers/maml_first_order_optimizer.py:82-115 with the task mean of

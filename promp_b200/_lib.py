@@ -18,7 +18,7 @@ EARLY_TERM_ENVS = (ENV_POINT, ENV_WALKER)        # env kinds whose paths end on 
 INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write env_infos channels
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE, OBJ_EXPLORE = 0, 1, 2, 3, 4
-BASELINE_ZERO, BASELINE_LINEAR_FEATURE = 0, 1
+BASELINE_ZERO, BASELINE_LINEAR_FEATURE, BASELINE_LINEAR_TIME, BASELINE_GIVEN = 0, 1, 2, 3
 # the policy / rollout `hidden` argument: width | activation flag (no flag = tanh)
 HIDDEN_WIDTH_MASK, ACT_RELU = 0xFF, 0x100
 
@@ -63,6 +63,10 @@ _SIGNATURES = {
     'promp_process_workspace_bytes_ragged': (c_int64, [c_int, c_int, c_int, c_int]),
     'promp_process_samples_ragged': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_double, c_double, c_double, c_int,
                                              c_int, c_int, _P, _P, _P, _P, _P, c_int64, _P]),
+    'promp_process_samples_given': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_double, c_double, c_int, c_int, _P, _P,
+                                            _P, _P, c_int64, _P]),
+    'promp_process_samples_ragged_given': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_double, c_double, c_int,
+                                                   c_int, _P, _P, _P, _P, c_int64, _P]),
     'promp_process_launch_info': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     'promp_adj_avg_rewards': (c_int, [c_int64, _P, c_double, c_double, _P, _P]),
     'promp_emaml_coeff': (c_int, [c_int, _P, _P, c_int, _P, _P]),
@@ -71,6 +75,8 @@ _SIGNATURES = {
     'promp_baseline_fit_workspace_bytes': (c_int64, [c_int, c_int, c_int]),
     'promp_baseline_fit': (c_int, [c_int, c_int, c_int, _P, _P, _P, c_double, _P, _P, _P, c_int64, _P]),
     'promp_baseline_predict': (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    'promp_baseline_fit_ex': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_double, _P, _P, _P, c_int64, _P]),
+    'promp_baseline_predict_ex': (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     'promp_policy_workspace_bytes': (c_int64, [c_int, c_int, c_int, c_int, c_int]),
     'promp_policy_grad': (c_int, [c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, _P, _P, c_int, c_int,
                                   c_float, c_float, c_float, c_int, c_float, _P, _P, c_float, _P, _P, c_int64, _P]),

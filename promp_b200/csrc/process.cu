@@ -28,6 +28,10 @@ constexpr int PS_RING = 4;          // TMA stages of the Gram loop (observation 
 constexpr int PS_SMEM_BUDGET = 160 * 1024;  // above this the sample arrays stay in the (L2-resident) workspace
 
 enum { PS_MODE_PROCESS = 0, PS_MODE_FIT_ONLY = 1 };
+// Baseline kind as a template argument of process_fused_kernel.  PS_KIND_RUNTIME: ZERO or LINEAR_FEATURE, chosen by
+// A.baseline_kind at run time (the kernels this file always had).  LINEAR_TIME and GIVEN are instantiations of their own,
+// so the code the two runtime kinds run is compiled exactly as before.
+constexpr int PS_KIND_RUNTIME = -1;
 
 #ifdef PROMP_EXP_CLOCKS
 __device__ unsigned long long g_proc_clk[16];
@@ -64,6 +68,7 @@ struct ProcArgs {
     int finish_cap;           // samples the finish stage can stage in shared memory (0: use ws64)
     int tt_cap;               // entries of the shared-memory time-feature table t/100 (covers every step of fixed-horizon paths)
     int pred_tile;            // samples per TMA tile of the predict stage (0: no TMA ring there)
+    const double* __restrict__ given;       // [M][NS] caller's baseline values (PROMP_BASELINE_GIVEN only)
 };
 __device__ __forceinline__ int n_paths_of(const ProcArgs& A, int m) { return (A.path_off && A.n_paths) ? __ldg(A.n_paths + m) : A.E; }
 __device__ __forceinline__ int path_begin(const ProcArgs& A, int m, int e) {
@@ -129,13 +134,18 @@ __device__ __forceinline__ double ordered_sum_ldcg(const double* p, int cnt, int
 // (one divide per table entry, exact like the reference), (ii) the serial scans run in blocks of 4 steps whose loads are
 // issued before the dependent DFMA chain, (iii) the Cholesky uses one rsqrt per column and multiplies by stored inverse
 // pivots, (iv) partials written by other CTAs are fetched with batched independent loads.
-template <bool STAGE_F, bool STAGE_L>
+// KIND (see PS_KIND_RUNTIME): LINEAR_TIME fits the 4 time features only (LinearTimeBaseline, linear_baseline.py:109-126):
+// no observation is read, the chunk partials are its 5 x 5 Gram matrix [Phi | y]^T [Phi | y] (padded into the same 4x4
+// block layout), and the prediction is the per-step table alone.  GIVEN reads the baseline values from A.given.
+template <bool STAGE_F, bool STAGE_L, int KIND = PS_KIND_RUNTIME>
 __global__ void __launch_bounds__(PS_THREADS, 3) process_fused_kernel(ProcArgs A) {
+    constexpr bool TIME = KIND == PROMP_BASELINE_LINEAR_TIME, GIVEN = KIND == PROMP_BASELINE_GIVEN;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int c = blockIdx.x, m = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
     const int E = n_paths_of(A, m), H = A.H, Do = A.Do, NS = A.NS;
-    const int F = 2 * Do + 4, NC = F + 1, nb = (NC + 3) >> 2, NCP = nb * 4, nblk = nb * (nb + 1) / 2;
-    const bool linear = A.baseline_kind == PROMP_BASELINE_LINEAR_FEATURE;
+    const int F = TIME ? 4 : 2 * Do + 4, NC = F + 1, nb = (NC + 3) >> 2, NCP = nb * 4, nblk = nb * (nb + 1) / 2;
+    const int T0 = TIME ? 0 : 2 * Do;                  // first time feature among the coefficients
+    const bool linear = !GIVEN && (TIME || A.baseline_kind == PROMP_BASELINE_LINEAR_FEATURE);
     const int e_lo = min(E, c * A.EPC), e_hi = min(E, e_lo + A.EPC);
     const float* __restrict__ obs = A.obs + (int64_t)m * NS * Do;
     const float* __restrict__ rew = A.rew ? A.rew + (int64_t)m * NS : nullptr;
@@ -242,8 +252,37 @@ __global__ void __launch_bounds__(PS_THREADS, 3) process_fused_kernel(ProcArgs A
     }
 
     PCLK(2);
+    if constexpr (TIME) {
+        // ---- time features only: thread-strided sums of f_a f_b (a <= b) and f_a y over the chunk, f = [t, t^2, t^3, 1]
+        double s[14];
+#pragma unroll
+        for (int k = 0; k < 14; ++k) s[k] = 0.0;
+        for (int i = tid; i < ns; i += PS_THREADS) {
+            const int n = n_lo + i;
+            const int step = tpos ? tpos[n] : n % H;
+            const double tt = step < A.tt_cap ? tt_s[step] : (double)step / 100.0;
+            const double f[4] = {tt, tt * tt, tt * tt * tt, 1.0}, y = val[i];
+            int k = 0;
+#pragma unroll
+            for (int a = 0; a < 4; ++a)
+#pragma unroll
+                for (int b = a; b < 4; ++b) s[k++] += f[a] * f[b];
+#pragma unroll
+            for (int a = 0; a < 4; ++a) s[10 + a] += f[a] * y;
+        }
+        const int op[14] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        block_reduce<14>(s, op, red);
+        double* gp = A.gram_p + ((int64_t)m * A.C + c) * PS_GP;
+        if (tid == 0) {
+#pragma unroll
+            for (int idx = 0; idx < 48; ++idx) {           // blocks (0,0), (0,1), (1,1) of the 8 x 8 layout (nb = 2)
+                const int b = idx >> 4, i = 4 * (b == 2) + ((idx >> 2) & 3), j = 4 * (b != 0) + (idx & 3);
+                const int lo = min(i, j), hi = max(i, j);
+                gp[idx] = hi < 4 ? s[lo * 4 - lo * (lo - 1) / 2 + (hi - lo)] : (hi == 4 && lo < 4) ? s[10 + lo] : 0.0;
+            }
+        }
+    } else if (linear) {
     // ---- partial Gram matrix over this chunk's samples (baselines/linear_baseline.py:66-73): thread = (4x4 block, group)
-    if (linear) {
         const int G = max(1, min(PS_THREADS / nblk, 8));
         const int blk = tid % nblk, g = tid / nblk;
         const bool active = g < G;
@@ -491,66 +530,71 @@ __global__ void __launch_bounds__(PS_THREADS, 3) process_fused_kernel(ProcArgs A
         __syncthreads();                                    // every thread is done with A / L before they become the ring
         for (int t = tid; t < A.tt_cap; t += PS_THREADS) {
             const double tt = tt_s[t];
-            tw[t] = fma(tt, wv[2 * Do], fma(tt * tt, wv[2 * Do + 1], fma(tt * tt * tt, wv[2 * Do + 2], wv[2 * Do + 3])));
+            tw[t] = fma(tt, wv[T0], fma(tt * tt, wv[T0 + 1], fma(tt * tt * tt, wv[T0 + 2], wv[T0 + 3])));
         }
         __syncthreads();
         auto time_part = [&](int n) {
             const int step = tpos ? tpos[n] : n % H;
             if (step < A.tt_cap) return tw[step];
             const double tt = (double)step / 100.0;          // beyond the table (very long variable-length paths)
-            return fma(tt, wv[2 * Do], fma(tt * tt, wv[2 * Do + 1], fma(tt * tt * tt, wv[2 * Do + 2], wv[2 * Do + 3])));
+            return fma(tt, wv[T0], fma(tt * tt, wv[T0 + 1], fma(tt * tt * tt, wv[T0 + 2], wv[T0 + 3])));
         };
-        // Observations of the whole task stream through a 2-stage TMA ring of A.pred_tile samples (re-using the tile / A / L
-        // area, which is dead by now): thread = one sample of the tile, row stride Do floats.
-        int n_done = 0;
-        const int PT = A.pred_tile;
-        if (STAGE_L && PT > 0 && N >= PT && ((reinterpret_cast<uintptr_t>(obs) & 15) == 0)) {
-            float* pring = reinterpret_cast<float*>(tile);
-            const int ptiles = N / PT, pfloats = PT * Do;
-            if (tid == 0) {
-                tma_load_1d(pring, obs, (uint32_t)pfloats * 4u, &s_bar_p[0]);
-                if (ptiles > 1) tma_load_1d(pring + pfloats, obs + pfloats, (uint32_t)pfloats * 4u, &s_bar_p[1]);
-            }
-            for (int t = 0; t < ptiles; ++t) {
-                tma_mbar_wait(&s_bar_p[t & 1], (uint32_t)((t >> 1) & 1));
-                if (tid < PT) {
-                    const float* src = pring + (t & 1) * pfloats + tid * Do;
-                    const int n = t * PT + tid;
-                    double b = time_part(n), b2 = 0.0, b3 = 0.0, b4 = 0.0;      // four chains: the fp64 FMA latency, not its
-                    int i = 0;                                                    // throughput, limits this loop
-                    for (; i + 1 < Do; i += 2) {
-                        const double c0 = fmin(fmax((double)src[i], -10.0), 10.0), c1 = fmin(fmax((double)src[i + 1], -10.0), 10.0);
-                        b = fma(c0, wv[i], b);
-                        b2 = fma(c0 * c0, wv[Do + i], b2);
-                        b3 = fma(c1, wv[i + 1], b3);
-                        b4 = fma(c1 * c1, wv[Do + i + 1], b4);
-                    }
-                    if (i < Do) {
-                        const double c0 = fmin(fmax((double)src[i], -10.0), 10.0);
-                        b = fma(c0, wv[i], b);
-                        b2 = fma(c0 * c0, wv[Do + i], b2);
-                    }
-                    bval[n] = (b + b2) + (b3 + b4);
+        if constexpr (TIME) {
+            for (int n = tid; n < N; n += PS_THREADS) bval[n] = time_part(n);
+        } else {
+            // Observations of the whole task stream through a 2-stage TMA ring of A.pred_tile samples (re-using the tile / A / L
+            // area, which is dead by now): thread = one sample of the tile, row stride Do floats.
+            int n_done = 0;
+            const int PT = A.pred_tile;
+            if (STAGE_L && PT > 0 && N >= PT && ((reinterpret_cast<uintptr_t>(obs) & 15) == 0)) {
+                float* pring = reinterpret_cast<float*>(tile);
+                const int ptiles = N / PT, pfloats = PT * Do;
+                if (tid == 0) {
+                    tma_load_1d(pring, obs, (uint32_t)pfloats * 4u, &s_bar_p[0]);
+                    if (ptiles > 1) tma_load_1d(pring + pfloats, obs + pfloats, (uint32_t)pfloats * 4u, &s_bar_p[1]);
                 }
-                __syncthreads();                  // stage (t & 1) consumed
-                if (tid == 0 && t + 2 < ptiles)
-                    tma_load_1d(pring + (t & 1) * pfloats, obs + (int64_t)(t + 2) * pfloats, (uint32_t)pfloats * 4u, &s_bar_p[t & 1]);
+                for (int t = 0; t < ptiles; ++t) {
+                    tma_mbar_wait(&s_bar_p[t & 1], (uint32_t)((t >> 1) & 1));
+                    if (tid < PT) {
+                        const float* src = pring + (t & 1) * pfloats + tid * Do;
+                        const int n = t * PT + tid;
+                        double b = time_part(n), b2 = 0.0, b3 = 0.0, b4 = 0.0;      // four chains: the fp64 FMA latency, not its
+                        int i = 0;                                                    // throughput, limits this loop
+                        for (; i + 1 < Do; i += 2) {
+                            const double c0 = fmin(fmax((double)src[i], -10.0), 10.0), c1 = fmin(fmax((double)src[i + 1], -10.0), 10.0);
+                            b = fma(c0, wv[i], b);
+                            b2 = fma(c0 * c0, wv[Do + i], b2);
+                            b3 = fma(c1, wv[i + 1], b3);
+                            b4 = fma(c1 * c1, wv[Do + i + 1], b4);
+                        }
+                        if (i < Do) {
+                            const double c0 = fmin(fmax((double)src[i], -10.0), 10.0);
+                            b = fma(c0, wv[i], b);
+                            b2 = fma(c0 * c0, wv[Do + i], b2);
+                        }
+                        bval[n] = (b + b2) + (b3 + b4);
+                    }
+                    __syncthreads();                  // stage (t & 1) consumed
+                    if (tid == 0 && t + 2 < ptiles)
+                        tma_load_1d(pring + (t & 1) * pfloats, obs + (int64_t)(t + 2) * pfloats, (uint32_t)pfloats * 4u, &s_bar_p[t & 1]);
+                }
+                n_done = ptiles * PT;
             }
-            n_done = ptiles * PT;
-        }
-        for (int n = n_done + tid; n < N; n += PS_THREADS) {      // rest (tail / no TMA): straight from global memory
-            const float* o = obs + (int64_t)n * Do;
-            double b = time_part(n);
-            for (int i = 0; i < Do; ++i) {
-                const double cl = fmin(fmax((double)__ldg(o + i), -10.0), 10.0);
-                b = fma(cl, wv[i], b);
-                b = fma(cl * cl, wv[Do + i], b);
+            for (int n = n_done + tid; n < N; n += PS_THREADS) {      // rest (tail / no TMA): straight from global memory
+                const float* o = obs + (int64_t)n * Do;
+                double b = time_part(n);
+                for (int i = 0; i < Do; ++i) {
+                    const double cl = fmin(fmax((double)__ldg(o + i), -10.0), 10.0);
+                    b = fma(cl, wv[i], b);
+                    b = fma(cl * cl, wv[Do + i], b);
+                }
+                bval[n] = b;
             }
-            bval[n] = b;
         }
     } else {
         if (A.mode == PS_MODE_FIT_ONLY) return;
-        for (int n = tid; n < N; n += PS_THREADS) bval[n] = 0.0;   // ZeroBaseline.predict
+        for (int n = tid; n < N; n += PS_THREADS)                  // ZeroBaseline.predict, or the caller's values
+            bval[n] = GIVEN ? __ldg(A.given + (int64_t)m * NS + n) : 0.0;
     }
     __syncthreads();
     PCLK(10);
@@ -665,9 +709,12 @@ __global__ void emaml_coeff_kernel(int M, const double* __restrict__ stats, cons
     }
 }
 
-// LinearFeatureBaseline.predict (baselines/linear_baseline.py:17-33) for a flat list of paths
+// LinearFeatureBaseline / LinearTimeBaseline (KIND) .predict (baselines/linear_baseline.py:17-33) for a flat list of paths
+template <int KIND>
 __global__ void baseline_predict_kernel(int n_paths, const int32_t* __restrict__ path_off, int Do, const float* __restrict__ obs,
                                         const double* __restrict__ coeffs, double* __restrict__ out) {
+    constexpr bool TIME = KIND == PROMP_BASELINE_LINEAR_TIME;
+    const int T0 = TIME ? 0 : 2 * Do;
     const int n_total = __ldg(path_off + n_paths);
     for (int n = blockIdx.x * blockDim.x + threadIdx.x; n < n_total; n += gridDim.x * blockDim.x) {
         int lo = 0, hi = n_paths;           // path containing sample n: path_off[lo] <= n < path_off[lo+1]
@@ -676,18 +723,20 @@ __global__ void baseline_predict_kernel(int n_paths, const int32_t* __restrict__
             if (__ldg(path_off + mid) <= n) lo = mid; else hi = mid;
         }
         const int step = n - __ldg(path_off + lo);
-        const float* o = obs + (int64_t)n * Do;
         double b = 0.0;
-        for (int i = 0; i < Do; ++i) {
-            const double cl = fmin(fmax((double)__ldg(o + i), -10.0), 10.0);
-            b = fma(cl, coeffs[i], b);
-            b = fma(cl * cl, coeffs[Do + i], b);
+        if constexpr (!TIME) {
+            const float* o = obs + (int64_t)n * Do;
+            for (int i = 0; i < Do; ++i) {
+                const double cl = fmin(fmax((double)__ldg(o + i), -10.0), 10.0);
+                b = fma(cl, coeffs[i], b);
+                b = fma(cl * cl, coeffs[Do + i], b);
+            }
         }
         const double tt = (double)step / 100.0;
-        b = fma(tt, coeffs[2 * Do], b);
-        b = fma(tt * tt, coeffs[2 * Do + 1], b);
-        b = fma(tt * tt * tt, coeffs[2 * Do + 2], b);
-        out[n] = b + coeffs[2 * Do + 3];
+        b = fma(tt, coeffs[T0], b);
+        b = fma(tt * tt, coeffs[T0 + 1], b);
+        b = fma(tt * tt * tt, coeffs[T0 + 2], b);
+        out[n] = b + coeffs[T0 + 3];
     }
 }
 
@@ -700,13 +749,15 @@ static int proc_tt_cap(int H, int NS, bool ragged) {
     const int n = ragged ? NS : H;
     return ((n < 1024 ? n : 1024) + 1) & ~1;      // even: keeps the areas behind the table 16-byte aligned
 }
-static size_t proc_smem_fixed(int Do, int tt_cap) {
-    const int NC = 2 * Do + 5, NCP = (NC + 3) / 4 * 4;
+// F: the kind's feature count (proc_features); kinds 0 and 1 size for 2*Do+4 as they always have
+static int proc_features(int Do, int kind) { return kind == PROMP_BASELINE_LINEAR_TIME ? 4 : 2 * Do + 4; }
+static size_t proc_smem_fixed(int F, int tt_cap) {
+    const int NC = F + 1, NCP = (NC + 3) / 4 * 4;
     const int u = 2 * PS_TS * NCP > PS_THREADS * 8 ? 2 * PS_TS * NCP : PS_THREADS * 8;      // tiles and scratch share one area
     return (size_t)(u + tt_cap) * 8;
 }
-static size_t proc_smem_finish_fixed(int Do) {
-    const int NC = 2 * Do + 5, NCP = (NC + 3) / 4 * 4, F = 2 * Do + 4, LD = F | 1;
+static size_t proc_smem_finish_fixed(int F) {
+    const int NC = F + 1, NCP = (NC + 3) / 4 * 4, LD = F | 1;
     return (size_t)(NCP * NCP + F * LD + (F * LD & 1) + PS_MAXCOL + 4) * 8;
 }
 struct ProcGeom {
@@ -719,30 +770,33 @@ struct ProcGeom {
 // Invariant: !stage_f implies !stage_l.  front - fin = round16(chunk_samples*12) + ring - proc_smem_finish_fixed(Do) - NS*12
 // with chunk_samples <= NS, and the Gram loop's TMA ring (PS_RING*PS_TS*Do*4 B) plus the 12 B of rounding is smaller than
 // the finish stage's fixed arrays for every obs_dim 1..19, so front < fin: when the front stage does not fit, neither does
-// the finish stage.  launch_process therefore has no <false, true> kernel.
-static ProcGeom proc_geom_for(int EPC, int E, int H, int Do, int NS, bool ragged) {
+// the finish stage.  launch_process therefore has no <false, true> kernel.  The time kind reads no observations: no ring
+// in either stage (and its finish stage's fixed arrays, 1056 B, still exceed the 12 B of rounding).
+static ProcGeom proc_geom_for(int EPC, int E, int H, int Do, int NS, bool ragged, int kind) {
     ProcGeom g;
+    const bool reads_obs = kind != PROMP_BASELINE_LINEAR_TIME;
+    const int F = proc_features(Do, kind);
     g.EPC = EPC;
     g.C = (E + EPC - 1) / EPC;
     g.tt_cap = proc_tt_cap(H, NS, ragged);
     const int chunk_samples = ragged ? NS : EPC * H;
-    const size_t fixed = proc_smem_fixed(Do, g.tt_cap);
-    const size_t ring = (size_t)PS_RING * PS_TS * Do * 4;                    // TMA stages of the Gram loop
+    const size_t fixed = proc_smem_fixed(F, g.tt_cap);
+    const size_t ring = reads_obs ? (size_t)PS_RING * PS_TS * Do * 4 : 0;   // TMA stages of the Gram loop
     size_t front = fixed + ((size_t)chunk_samples * PS_SMEM_SAMPLES_BYTES + 15) / 16 * 16 + ring;
-    size_t fin = fixed + proc_smem_finish_fixed(Do) + (size_t)NS * PS_SMEM_SAMPLES_BYTES;
+    size_t fin = fixed + proc_smem_finish_fixed(F) + (size_t)NS * PS_SMEM_SAMPLES_BYTES;
     // predict ring: 2 stages of pred_tile samples inside the (dead) tile / A / L area
-    {
-        const int NC = 2 * Do + 5, NCP = (NC + 3) / 4 * 4;
-        const int F = 2 * Do + 4, LD = F | 1;
+    g.pred_tile = 0;
+    if (reads_obs) {
+        const int NC = F + 1, NCP = (NC + 3) / 4 * 4;
+        const int LD = F | 1;
         const size_t avail = (size_t)(2 * PS_TS * NCP + NCP * NCP + F * LD) * 8;
-        g.pred_tile = 0;
         for (int pt = 256; pt >= 32; pt >>= 1)
             if ((size_t)2 * pt * Do * 4 <= avail) { g.pred_tile = pt; break; }
     }
     g.stage_f = front <= (size_t)PS_SMEM_BUDGET;
     g.stage_l = fin <= (size_t)PS_SMEM_BUDGET;
     if (!g.stage_f) front = fixed;
-    if (!g.stage_l) fin = fixed + proc_smem_finish_fixed(Do);
+    if (!g.stage_l) fin = fixed + proc_smem_finish_fixed(F);
     g.chunk_cap = g.stage_f ? chunk_samples : 0;
     g.finish_cap = g.stage_l ? NS : 0;
     g.smem = (front > fin ? front : fin) + 16;
@@ -751,21 +805,22 @@ static ProcGeom proc_geom_for(int EPC, int E, int H, int Do, int NS, bool ragged
 // Chunking: ~4 CTAs per SM worth of chunks (the front stage is issue / latency-bound at 8-16 resident warps per SM, so
 // short chunks on many CTAs beat one exact wave of longer ones: measured 33 vs 38 us at 40x20x100), never more than one
 // CTA per path.
-static ProcGeom proc_geom(int M, int E, int H, int Do, int NS, bool ragged) {
+static ProcGeom proc_geom(int M, int E, int H, int Do, int NS, bool ragged, int kind) {
     int target = (4 * PROMP_NUM_SMS + M - 1) / M;
     if (target > E) target = E;
     if (target < 1) target = 1;
     const int EPC = (E + target - 1) / target;
-    return proc_geom_for(EPC, E, H, Do, NS, ragged);
+    return proc_geom_for(EPC, E, H, Do, NS, ragged, kind);
 }
 
 struct ProcLayout {
     ProcGeom g;
     int64_t off_gram, off_stat, off_ws64, off_tpos, total;
 };
-static ProcLayout proc_layout(int M, int E, int H, int Do, int NS, bool ragged) {
+// The offsets depend on C only, which no kind changes: one workspace size serves every kind.
+static ProcLayout proc_layout(int M, int E, int H, int Do, int NS, bool ragged, int kind) {
     ProcLayout L;
-    L.g = proc_geom(M, E, H, Do, NS, ragged);
+    L.g = proc_geom(M, E, H, Do, NS, ragged, kind);
     // arrival tickets: a FIXED-size header (grid.y <= 65535 tasks), so a workspace shared by launches of different
     // shapes never finds stale partials where a later layout expects zeroed tickets
     int64_t o = 65536 * 4;
@@ -777,18 +832,25 @@ static ProcLayout proc_layout(int M, int E, int H, int Do, int NS, bool ragged) 
     return L;
 }
 
+template <int KIND>
+static void (*proc_kernel(const ProcGeom& g))(ProcArgs) {
+    return g.stage_f ? (g.stage_l ? process_fused_kernel<true, true, KIND> : process_fused_kernel<true, false, KIND>)
+                     : process_fused_kernel<false, false, KIND>;
+}
+
 static int launch_process(ProcArgs& A, const ProcGeom& g, cudaStream_t stream) {
     A.C = g.C; A.EPC = g.EPC; A.chunk_cap = g.chunk_cap; A.finish_cap = g.finish_cap; A.tt_cap = g.tt_cap;
     A.pred_tile = g.pred_tile;
     PROMP_REQUIRE(g.stage_f || !g.stage_l, "process_fused_kernel: finish stage staged without a staged front stage "
                   "(M=%d E=%d Do=%d NS=%d); proc_geom_for's invariant is broken", A.M, A.E, A.Do, A.NS);
-    auto kern = g.stage_f ? (g.stage_l ? process_fused_kernel<true, true> : process_fused_kernel<true, false>)
-                          : process_fused_kernel<false, false>;
-    static size_t configured[3] = {0, 0, 0};
+    const int slot = A.baseline_kind == PROMP_BASELINE_LINEAR_TIME ? 1 : A.baseline_kind == PROMP_BASELINE_GIVEN ? 2 : 0;
+    auto kern = slot == 1 ? proc_kernel<PROMP_BASELINE_LINEAR_TIME>(g)
+              : slot == 2 ? proc_kernel<PROMP_BASELINE_GIVEN>(g) : proc_kernel<PS_KIND_RUNTIME>(g);
+    static size_t configured[3][3] = {};
     const int which = g.stage_f ? (g.stage_l ? 2 : 1) : 0;
-    if (g.smem > configured[which]) {
+    if (g.smem > configured[slot][which]) {
         PROMP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)g.smem));
-        configured[which] = g.smem;
+        configured[slot][which] = g.smem;
     }
     kern<<<dim3(A.C, A.M), PS_THREADS, g.smem, stream>>>(A);
     PROMP_LAUNCH_CHECK("process_fused_kernel");
@@ -800,32 +862,30 @@ extern "C" int promp_process_launch_info(int M, int max_paths, int H, int obs_di
     PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "promp_process_launch_info: obs_dim %d too large (max %d)", obs_dim,
                   (PS_MAXCOL - 5) / 2);
     PROMP_REQUIRE(ragged || (H > 0 && NS == max_paths * H), "promp_process_launch_info: fixed horizon needs NS = E*H");
-    const ProcGeom g = proc_geom(M, max_paths, ragged ? 0 : H, obs_dim, NS, ragged != 0);
+    const ProcGeom g = proc_geom(M, max_paths, ragged ? 0 : H, obs_dim, NS, ragged != 0, PROMP_BASELINE_LINEAR_FEATURE);
     const int32_t v[8] = {g.C, g.EPC, g.chunk_cap, g.finish_cap, g.tt_cap, g.pred_tile, g.stage_f ? 1 : 0, g.stage_l ? 1 : 0};
     for (int i = 0; i < 8; ++i) out[i] = v[i];
     return PROMP_OK;
 }
 
 extern "C" int64_t promp_process_workspace_bytes(int M, int E, int H, int obs_dim) {
-    return proc_layout(M, E, H, obs_dim, E * H, false).total;
+    return proc_layout(M, E, H, obs_dim, E * H, false, PROMP_BASELINE_LINEAR_FEATURE).total;
 }
 
-extern "C" int promp_process_samples(int M, int E, int H, int obs_dim, const float* obs, const float* rew,
-                                     double discount, double gae_lambda, double reg_coeff, int baseline_kind,
-                                     int normalize_adv, int positive_adv, float* returns, float* adv, double* coeffs,
-                                     double* stats, void* workspace, int64_t workspace_bytes, void* stream) {
-    PROMP_REQUIRE(M > 0 && E > 0 && H > 0 && obs_dim > 0, "promp_process_samples: dimensions must be positive");
-    PROMP_REQUIRE(M <= 65535, "promp_process_samples: M=%d exceeds the grid.y limit", M);
-    PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "promp_process_samples: obs_dim %d too large (max %d)", obs_dim,
-                  (PS_MAXCOL - 5) / 2);
-    PROMP_REQUIRE(obs && rew && returns && adv && workspace, "promp_process_samples: null pointer argument");
-    PROMP_REQUIRE(baseline_kind == PROMP_BASELINE_ZERO || baseline_kind == PROMP_BASELINE_LINEAR_FEATURE,
-                  "promp_process_samples: unknown baseline kind %d", baseline_kind);
+// kind: ZERO, LINEAR_FEATURE, LINEAR_TIME, or GIVEN with `given` set (obs is not read by the last two)
+static int process_fixed(const char* who, int M, int E, int H, int obs_dim, const float* obs, const float* rew,
+                         const double* given, double discount, double gae_lambda, double reg_coeff, int baseline_kind,
+                         int normalize_adv, int positive_adv, float* returns, float* adv, double* coeffs, double* stats,
+                         void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(M > 0 && E > 0 && H > 0 && obs_dim > 0, "%s: dimensions must be positive", who);
+    PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit", who, M);
+    PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "%s: obs_dim %d too large (max %d)", who, obs_dim, (PS_MAXCOL - 5) / 2);
+    PROMP_REQUIRE(obs && rew && returns && adv && workspace, "%s: null pointer argument", who);
     PROMP_REQUIRE(discount >= 0.0 && discount <= 1.0 && gae_lambda >= 0.0 && gae_lambda <= 1.0,
-                  "promp_process_samples: discount and gae_lambda must be in [0,1]");   // samplers/base.py:56-57
-    const ProcLayout L = proc_layout(M, E, H, obs_dim, E * H, false);
+                  "%s: discount and gae_lambda must be in [0,1]", who);   // samplers/base.py:56-57
+    const ProcLayout L = proc_layout(M, E, H, obs_dim, E * H, false, baseline_kind);
     if (workspace_bytes < L.total) {
-        set_error("promp_process_samples: workspace too small (%lld < %lld bytes)", (long long)workspace_bytes, (long long)L.total);
+        set_error("%s: workspace too small (%lld < %lld bytes)", who, (long long)workspace_bytes, (long long)L.total);
         return PROMP_ERR_WORKSPACE;
     }
     unsigned char* w = (unsigned char*)workspace;
@@ -837,8 +897,30 @@ extern "C" int promp_process_samples(int M, int E, int H, int obs_dim, const flo
     A.counters = (unsigned int*)w; A.gram_p = (double*)(w + L.off_gram); A.stat_p = (double*)(w + L.off_stat);
     A.ws64 = (double*)(w + L.off_ws64);
     A.path_off = nullptr; A.n_paths = nullptr; A.NS = E * H; A.tpos = nullptr;
-    A.target = nullptr; A.mode = PS_MODE_PROCESS;
+    A.target = nullptr; A.mode = PS_MODE_PROCESS; A.given = given;
     return launch_process(A, L.g, (cudaStream_t)stream);
+}
+
+extern "C" int promp_process_samples(int M, int E, int H, int obs_dim, const float* obs, const float* rew,
+                                     double discount, double gae_lambda, double reg_coeff, int baseline_kind,
+                                     int normalize_adv, int positive_adv, float* returns, float* adv, double* coeffs,
+                                     double* stats, void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(baseline_kind == PROMP_BASELINE_ZERO || baseline_kind == PROMP_BASELINE_LINEAR_FEATURE ||
+                  baseline_kind == PROMP_BASELINE_LINEAR_TIME, "promp_process_samples: unknown baseline kind %d", baseline_kind);
+    return process_fixed("promp_process_samples", M, E, H, obs_dim, obs, rew, nullptr, discount, gae_lambda, reg_coeff,
+                         baseline_kind, normalize_adv, positive_adv, returns, adv, coeffs, stats, workspace, workspace_bytes,
+                         stream);
+}
+
+// MetaSampleProcessor with a host baseline object (samplers/base.py:99-108): the caller's predict(path) values, GAE onwards
+extern "C" int promp_process_samples_given(int M, int E, int H, int obs_dim, const float* obs, const float* rew,
+                                           const double* baseline_values, double discount, double gae_lambda, int normalize_adv,
+                                           int positive_adv, float* returns, float* adv, double* stats,
+                                           void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(baseline_values, "promp_process_samples_given: null baseline_values");
+    return process_fixed("promp_process_samples_given", M, E, H, obs_dim, obs, rew, baseline_values, discount, gae_lambda,
+                         0.0, PROMP_BASELINE_GIVEN, normalize_adv, positive_adv, returns, adv, nullptr, stats, workspace,
+                         workspace_bytes, stream);
 }
 
 extern "C" int promp_adj_avg_rewards(int64_t n, const float* rew, double mean, double std, float* out, void* stream) {
@@ -873,26 +955,23 @@ extern "C" int promp_emaml_finish(int M, const double* stats, const int32_t* n_v
 
 // ---- variable-length paths: same kernel driven by a per-task path table ------------------------------------------
 extern "C" int64_t promp_process_workspace_bytes_ragged(int M, int max_paths, int max_samples, int obs_dim) {
-    return proc_layout(M, max_paths, 0, obs_dim, max_samples, true).total;
+    return proc_layout(M, max_paths, 0, obs_dim, max_samples, true, PROMP_BASELINE_LINEAR_FEATURE).total;
 }
 
-extern "C" int promp_process_samples_ragged(int M, int max_paths, int max_samples, int obs_dim, const float* obs,
-                                            const float* rew, const int32_t* path_off, const int32_t* n_paths, double discount,
-                                            double gae_lambda, double reg_coeff, int baseline_kind, int normalize_adv,
-                                            int positive_adv, float* returns, float* adv, double* coeffs, double* stats,
-                                            void* workspace, int64_t workspace_bytes, void* stream) {
-    PROMP_REQUIRE(M > 0 && max_paths > 0 && max_samples > 0 && obs_dim > 0, "promp_process_samples_ragged: dimensions must be positive");
-    PROMP_REQUIRE(M <= 65535, "promp_process_samples_ragged: M=%d exceeds the grid.y limit", M);
-    PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "promp_process_samples_ragged: obs_dim %d too large (max %d)", obs_dim,
-                  (PS_MAXCOL - 5) / 2);
-    PROMP_REQUIRE(obs && rew && returns && adv && workspace && path_off && n_paths, "promp_process_samples_ragged: null pointer argument");
-    PROMP_REQUIRE(baseline_kind == PROMP_BASELINE_ZERO || baseline_kind == PROMP_BASELINE_LINEAR_FEATURE,
-                  "promp_process_samples_ragged: unknown baseline kind %d", baseline_kind);
+static int process_ragged(const char* who, int M, int max_paths, int max_samples, int obs_dim, const float* obs,
+                          const float* rew, const int32_t* path_off, const int32_t* n_paths, const double* given,
+                          double discount, double gae_lambda, double reg_coeff, int baseline_kind, int normalize_adv,
+                          int positive_adv, float* returns, float* adv, double* coeffs, double* stats,
+                          void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(M > 0 && max_paths > 0 && max_samples > 0 && obs_dim > 0, "%s: dimensions must be positive", who);
+    PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit", who, M);
+    PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "%s: obs_dim %d too large (max %d)", who, obs_dim, (PS_MAXCOL - 5) / 2);
+    PROMP_REQUIRE(obs && rew && returns && adv && workspace && path_off && n_paths, "%s: null pointer argument", who);
     PROMP_REQUIRE(discount >= 0.0 && discount <= 1.0 && gae_lambda >= 0.0 && gae_lambda <= 1.0,
-                  "promp_process_samples_ragged: discount and gae_lambda must be in [0,1]");
-    const ProcLayout L = proc_layout(M, max_paths, 0, obs_dim, max_samples, true);
+                  "%s: discount and gae_lambda must be in [0,1]", who);
+    const ProcLayout L = proc_layout(M, max_paths, 0, obs_dim, max_samples, true, baseline_kind);
     if (workspace_bytes < L.total) {
-        set_error("promp_process_samples_ragged: workspace too small (%lld < %lld bytes)", (long long)workspace_bytes, (long long)L.total);
+        set_error("%s: workspace too small (%lld < %lld bytes)", who, (long long)workspace_bytes, (long long)L.total);
         return PROMP_ERR_WORKSPACE;
     }
     unsigned char* w = (unsigned char*)workspace;
@@ -905,22 +984,50 @@ extern "C" int promp_process_samples_ragged(int M, int max_paths, int max_sample
     A.ws64 = (double*)(w + L.off_ws64);
     A.path_off = path_off; A.n_paths = n_paths; A.NS = max_samples;
     A.tpos = (int32_t*)(w + L.off_tpos);
-    A.target = nullptr; A.mode = PS_MODE_PROCESS;
+    A.target = nullptr; A.mode = PS_MODE_PROCESS; A.given = given;
     return launch_process(A, L.g, (cudaStream_t)stream);
 }
 
-// ---- standalone LinearFeatureBaseline.fit / predict (baselines/linear_baseline.py:55-77, 17-33) --------------------
-extern "C" int64_t promp_baseline_fit_workspace_bytes(int n_paths, int n_samples, int obs_dim) {
-    return proc_layout(1, n_paths, 0, obs_dim, n_samples, true).total;
+extern "C" int promp_process_samples_ragged(int M, int max_paths, int max_samples, int obs_dim, const float* obs,
+                                            const float* rew, const int32_t* path_off, const int32_t* n_paths, double discount,
+                                            double gae_lambda, double reg_coeff, int baseline_kind, int normalize_adv,
+                                            int positive_adv, float* returns, float* adv, double* coeffs, double* stats,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(baseline_kind == PROMP_BASELINE_ZERO || baseline_kind == PROMP_BASELINE_LINEAR_FEATURE ||
+                  baseline_kind == PROMP_BASELINE_LINEAR_TIME, "promp_process_samples_ragged: unknown baseline kind %d",
+                  baseline_kind);
+    return process_ragged("promp_process_samples_ragged", M, max_paths, max_samples, obs_dim, obs, rew, path_off, n_paths,
+                          nullptr, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv, returns, adv,
+                          coeffs, stats, workspace, workspace_bytes, stream);
 }
 
-extern "C" int promp_baseline_fit(int n_paths, int n_samples, int obs_dim, const float* obs, const double* target,
-                                  const int32_t* path_off, double reg_coeff, double* coeffs, double* reg_used,
-                                  void* workspace, int64_t workspace_bytes, void* stream) {
+extern "C" int promp_process_samples_ragged_given(int M, int max_paths, int max_samples, int obs_dim, const float* obs,
+                                                  const float* rew, const int32_t* path_off, const int32_t* n_paths,
+                                                  const double* baseline_values, double discount, double gae_lambda,
+                                                  int normalize_adv, int positive_adv, float* returns, float* adv,
+                                                  double* stats, void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(baseline_values, "promp_process_samples_ragged_given: null baseline_values");
+    return process_ragged("promp_process_samples_ragged_given", M, max_paths, max_samples, obs_dim, obs, rew, path_off,
+                          n_paths, baseline_values, discount, gae_lambda, 0.0, PROMP_BASELINE_GIVEN, normalize_adv,
+                          positive_adv, returns, adv, nullptr, stats, workspace, workspace_bytes, stream);
+}
+
+// ---- standalone LinearFeatureBaseline / LinearTimeBaseline .fit / predict (baselines/linear_baseline.py:55-77, 17-33) ---
+extern "C" int64_t promp_baseline_fit_workspace_bytes(int n_paths, int n_samples, int obs_dim) {
+    return proc_layout(1, n_paths, 0, obs_dim, n_samples, true, PROMP_BASELINE_LINEAR_FEATURE).total;
+}
+
+// kind: LINEAR_FEATURE or LINEAR_TIME (LinearTimeBaseline, linear_baseline.py:109-126; obs is not read and may be NULL)
+extern "C" int promp_baseline_fit_ex(int kind, int n_paths, int n_samples, int obs_dim, const float* obs, const double* target,
+                                     const int32_t* path_off, double reg_coeff, double* coeffs, double* reg_used,
+                                     void* workspace, int64_t workspace_bytes, void* stream) {
+    PROMP_REQUIRE(kind == PROMP_BASELINE_LINEAR_FEATURE || kind == PROMP_BASELINE_LINEAR_TIME,
+                  "promp_baseline_fit: unknown baseline kind %d", kind);
     PROMP_REQUIRE(n_paths > 0 && n_samples > 0 && obs_dim > 0, "promp_baseline_fit: dimensions must be positive");
     PROMP_REQUIRE(2 * obs_dim + 5 <= PS_MAXCOL, "promp_baseline_fit: obs_dim %d too large (max %d)", obs_dim, (PS_MAXCOL - 5) / 2);
-    PROMP_REQUIRE(obs && target && path_off && coeffs && workspace, "promp_baseline_fit: null pointer argument");
-    const ProcLayout L = proc_layout(1, n_paths, 0, obs_dim, n_samples, true);
+    PROMP_REQUIRE((obs || kind == PROMP_BASELINE_LINEAR_TIME) && target && path_off && coeffs && workspace,
+                  "promp_baseline_fit: null pointer argument");
+    const ProcLayout L = proc_layout(1, n_paths, 0, obs_dim, n_samples, true, kind);
     if (workspace_bytes < L.total) {
         set_error("promp_baseline_fit: workspace too small (%lld < %lld bytes)", (long long)workspace_bytes, (long long)L.total);
         return PROMP_ERR_WORKSPACE;
@@ -930,7 +1037,7 @@ extern "C" int promp_baseline_fit(int n_paths, int n_samples, int obs_dim, const
     ProcArgs A{};
     A.M = 1; A.E = n_paths; A.H = 0; A.Do = obs_dim; A.obs = obs; A.rew = nullptr;
     A.discount = 0.0; A.gae_lambda = 0.0; A.reg_coeff = reg_coeff;
-    A.baseline_kind = PROMP_BASELINE_LINEAR_FEATURE; A.normalize_adv = 0; A.positive_adv = 0;
+    A.baseline_kind = kind; A.normalize_adv = 0; A.positive_adv = 0;
     A.returns = nullptr; A.adv = nullptr; A.coeffs = coeffs; A.stats = nullptr;
     A.counters = (unsigned int*)w; A.gram_p = (double*)(w + L.off_gram); A.stat_p = (double*)(w + L.off_stat);
     A.ws64 = (double*)(w + L.off_ws64);
@@ -942,16 +1049,34 @@ extern "C" int promp_baseline_fit(int n_paths, int n_samples, int obs_dim, const
     return launch_process(A, L.g, (cudaStream_t)stream);
 }
 
-extern "C" int promp_baseline_predict(int n_paths, int n_samples, int obs_dim, const float* obs, const int32_t* path_off,
-                                      const double* coeffs, double* out, void* stream) {
+extern "C" int promp_baseline_fit(int n_paths, int n_samples, int obs_dim, const float* obs, const double* target,
+                                  const int32_t* path_off, double reg_coeff, double* coeffs, double* reg_used,
+                                  void* workspace, int64_t workspace_bytes, void* stream) {
+    return promp_baseline_fit_ex(PROMP_BASELINE_LINEAR_FEATURE, n_paths, n_samples, obs_dim, obs, target, path_off, reg_coeff,
+                                 coeffs, reg_used, workspace, workspace_bytes, stream);
+}
+
+extern "C" int promp_baseline_predict_ex(int kind, int n_paths, int n_samples, int obs_dim, const float* obs,
+                                         const int32_t* path_off, const double* coeffs, double* out, void* stream) {
+    PROMP_REQUIRE(kind == PROMP_BASELINE_LINEAR_FEATURE || kind == PROMP_BASELINE_LINEAR_TIME,
+                  "promp_baseline_predict: unknown baseline kind %d", kind);
     PROMP_REQUIRE(n_paths > 0 && n_samples > 0 && obs_dim > 0, "promp_baseline_predict: dimensions must be positive");
-    PROMP_REQUIRE(obs && path_off && coeffs && out, "promp_baseline_predict: null pointer argument");
+    PROMP_REQUIRE((obs || kind == PROMP_BASELINE_LINEAR_TIME) && path_off && coeffs && out,
+                  "promp_baseline_predict: null pointer argument");
     const int bs = 256;
     int grid = (n_samples + bs - 1) / bs;
     if (grid > PROMP_NUM_SMS * 8) grid = PROMP_NUM_SMS * 8;
-    baseline_predict_kernel<<<grid, bs, 0, (cudaStream_t)stream>>>(n_paths, path_off, obs_dim, obs, coeffs, out);
+    auto kern = kind == PROMP_BASELINE_LINEAR_TIME ? baseline_predict_kernel<PROMP_BASELINE_LINEAR_TIME>
+                                                   : baseline_predict_kernel<PROMP_BASELINE_LINEAR_FEATURE>;
+    kern<<<grid, bs, 0, (cudaStream_t)stream>>>(n_paths, path_off, obs_dim, obs, coeffs, out);
     PROMP_LAUNCH_CHECK("baseline_predict_kernel");
     return PROMP_OK;
+}
+
+extern "C" int promp_baseline_predict(int n_paths, int n_samples, int obs_dim, const float* obs, const int32_t* path_off,
+                                      const double* coeffs, double* out, void* stream) {
+    return promp_baseline_predict_ex(PROMP_BASELINE_LINEAR_FEATURE, n_paths, n_samples, obs_dim, obs, path_off, coeffs, out,
+                                     stream);
 }
 
 #ifdef PROMP_EXP_CLOCKS

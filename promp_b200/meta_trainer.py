@@ -91,6 +91,10 @@ class Trainer(object):
         from promp_b200.samplers.device_data import PhaseData
         sampler, proc, algo, policy = self.sampler, self.sample_processor, self.algo, self.policy
         assert sampler._fused_ok(), "graph mode needs the fused rollout path"
+        if getattr(proc.baseline, 'device_kind', None) is None:
+            raise ValueError("use_cuda_graph=True needs a device baseline (LinearFeatureBaseline, LinearTimeBaseline, "
+                             "ZeroBaseline): %r fits and predicts on the host, which a CUDA graph cannot replay; "
+                             "use use_cuda_graph=False or 'auto'" % (proc.baseline,))
         assert hasattr(algo, 'optimize_phases'), "graph mode needs an algorithm with a device-only outer step (ProMP, TRPOMAML)"
         S = self.num_inner_grad_steps + 1
         M, E, H = sampler.meta_batch_size, sampler.envs_per_task, sampler.max_path_length
@@ -247,10 +251,12 @@ class Trainer(object):
         return step
 
     def graph_capturable(self):
-        """True when a meta-iteration has no data-dependent host decision: fused fixed-horizon rollouts and an algorithm
-        with a device-only outer step (ProMP - its adaptive inner-KL coefficient rule runs on the device - and TRPO-MAML)."""
+        """True when a meta-iteration has no data-dependent host decision: fused fixed-horizon rollouts, a device baseline
+        (not a host baseline object) and an algorithm with a device-only outer step (ProMP - its adaptive inner-KL
+        coefficient rule runs on the device - and TRPO-MAML)."""
         return bool(self.sampler._fused_ok() and hasattr(self.algo, 'optimize_phases')
-                    and getattr(self.algo, 'graph_capturable', True))
+                    and getattr(self.algo, 'graph_capturable', True)
+                    and getattr(self.baseline, 'device_kind', None) is not None)
 
     def train(self):
         """meta_trainer.py:59-152.  The default entry point of a run script."""

@@ -2,7 +2,9 @@
 
 Mirrors meta_policy_search/samplers/meta_sample_processor.py:6-49 and samplers/base.py:33-173
 (constructor arguments, `.baseline`, process_samples(paths_meta_batch, log, log_prefix) -> list of M
-dicts with the 8 keys).  All numerics run in promp_process_samples (one CTA per task).
+dicts with the 8 keys).  All numerics run in promp_process_samples (one CTA per task).  A baseline object without a
+`device_kind` (any object with fit / predict, as the reference accepts) is fitted and evaluated on the host; the returns
+before it and the GAE, normalisation and statistics after it still run on the device.
 """
 import numpy as np
 
@@ -12,11 +14,12 @@ from promp_b200.utils import logger
 
 
 def _baseline_kind(baseline):
-    kind = getattr(baseline, 'device_kind', None)
-    if kind is None:
-        raise TypeError("promp_b200 implements LinearFeatureBaseline and ZeroBaseline on the device; got %r "
-                        "(no CPU fallback)" % (baseline,))
-    return kind
+    """The processing kernel's baseline kind, or None for a baseline object whose fit / predict run on the host."""
+    return getattr(baseline, 'device_kind', None)
+
+
+def _coeff_width(baseline_kind, obs_dim):
+    return 4 if baseline_kind == _lib.BASELINE_LINEAR_TIME else 2 * obs_dim + 4
 
 
 def _phase_from_host_paths(paths_meta_batch, device):
@@ -108,87 +111,139 @@ def _zeroed_workspace(nbytes, dev):
     return ws
 
 
-def run_process_kernel(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv):
+def run_process_kernel(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv, given=None):
+    """One launch of the processing kernel on `phase`.  baseline_kind BASELINE_GIVEN takes the baseline values from
+    `given` (float64 [M, N] device tensor in the phase's sample layout) and writes no coefficients."""
     import torch
     if isinstance(phase, RaggedPhaseData):
-        return _run_process_kernel_ragged(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv)
+        return _run_process_kernel_ragged(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv,
+                                          given)
     M, E, H, Do = phase.M, phase.E, phase.H, phase.obs_dim
     dev = phase.obs.device
     if phase.returns is None:
         phase.returns = torch.empty(M, E * H, dtype=torch.float32, device=dev)
         phase.adv = torch.empty(M, E * H, dtype=torch.float32, device=dev)
-        # both are fully written by the kernels (coeffs only by the linear-feature baseline): no fill launches
-        phase.coeffs = (torch.empty if baseline_kind == 1 else torch.zeros)(M, 2 * Do + 4, dtype=torch.float64, device=dev)
         phase.stats = torch.empty(M, 8, dtype=torch.float64, device=dev)
+    width = _coeff_width(baseline_kind, Do)
+    if phase.coeffs is None or phase.coeffs.shape[1] != width:
+        # fully written by the kernel for the linear baselines: no fill launch
+        fitted = baseline_kind in (_lib.BASELINE_LINEAR_FEATURE, _lib.BASELINE_LINEAR_TIME)
+        phase.coeffs = (torch.empty if fitted else torch.zeros)(M, width, dtype=torch.float64, device=dev)
     nbytes = _lib.load().promp_process_workspace_bytes(M, E, H, Do)
     ws = _zeroed_workspace(nbytes, dev)
-    _lib.call('promp_process_samples', M, E, H, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew), float(discount),
-              float(gae_lambda), float(reg_coeff), int(baseline_kind), int(bool(normalize_adv)), int(bool(positive_adv)),
-              _lib.ptr(phase.returns), _lib.ptr(phase.adv), _lib.ptr(phase.coeffs), _lib.ptr(phase.stats),
-              _lib.ptr(ws), ws.numel() * 8, _lib.stream())
+    if baseline_kind == _lib.BASELINE_GIVEN:
+        _lib.call('promp_process_samples_given', M, E, H, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew), _lib.ptr(given),
+                  float(discount), float(gae_lambda), int(bool(normalize_adv)), int(bool(positive_adv)),
+                  _lib.ptr(phase.returns), _lib.ptr(phase.adv), _lib.ptr(phase.stats), _lib.ptr(ws), ws.numel() * 8,
+                  _lib.stream())
+    else:
+        _lib.call('promp_process_samples', M, E, H, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew), float(discount),
+                  float(gae_lambda), float(reg_coeff), int(baseline_kind), int(bool(normalize_adv)), int(bool(positive_adv)),
+                  _lib.ptr(phase.returns), _lib.ptr(phase.adv), _lib.ptr(phase.coeffs), _lib.ptr(phase.stats),
+                  _lib.ptr(ws), ws.numel() * 8, _lib.stream())
     phase.adj_avg_rewards = None
     phase._explore_adv = None
     phase.invalidate_host()
 
 
-def _run_process_kernel_ragged(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv):
+def _run_process_kernel_ragged(phase, discount, gae_lambda, reg_coeff, baseline_kind, normalize_adv, positive_adv,
+                               given=None):
     import torch
     M, Pmax, N, Do = phase.M, phase.E, phase.N, phase.obs_dim
     dev = phase.obs.device
     if phase.returns is None:
         phase.returns = torch.zeros(M, N, dtype=torch.float32, device=dev)
         phase.adv = torch.zeros(M, N, dtype=torch.float32, device=dev)
-        phase.coeffs = torch.zeros(M, 2 * Do + 4, dtype=torch.float64, device=dev)
         phase.stats = torch.zeros(M, 8, dtype=torch.float64, device=dev)
+    width = _coeff_width(baseline_kind, Do)
+    if phase.coeffs is None or phase.coeffs.shape[1] != width:
+        phase.coeffs = torch.zeros(M, width, dtype=torch.float64, device=dev)
     nbytes = _lib.load().promp_process_workspace_bytes_ragged(M, Pmax, N, Do)
     ws = _zeroed_workspace(nbytes, dev)
-    _lib.call('promp_process_samples_ragged', M, Pmax, N, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew), _lib.ptr(phase.path_off),
-              _lib.ptr(phase.n_paths), float(discount), float(gae_lambda), float(reg_coeff), int(baseline_kind),
-              int(bool(normalize_adv)), int(bool(positive_adv)), _lib.ptr(phase.returns), _lib.ptr(phase.adv),
-              _lib.ptr(phase.coeffs), _lib.ptr(phase.stats), _lib.ptr(ws), ws.numel() * 8, _lib.stream())
+    if baseline_kind == _lib.BASELINE_GIVEN:
+        _lib.call('promp_process_samples_ragged_given', M, Pmax, N, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew),
+                  _lib.ptr(phase.path_off), _lib.ptr(phase.n_paths), _lib.ptr(given), float(discount), float(gae_lambda),
+                  int(bool(normalize_adv)), int(bool(positive_adv)), _lib.ptr(phase.returns), _lib.ptr(phase.adv),
+                  _lib.ptr(phase.stats), _lib.ptr(ws), ws.numel() * 8, _lib.stream())
+    else:
+        _lib.call('promp_process_samples_ragged', M, Pmax, N, Do, _lib.ptr(phase.obs), _lib.ptr(phase.rew),
+                  _lib.ptr(phase.path_off), _lib.ptr(phase.n_paths), float(discount), float(gae_lambda), float(reg_coeff),
+                  int(baseline_kind), int(bool(normalize_adv)), int(bool(positive_adv)), _lib.ptr(phase.returns),
+                  _lib.ptr(phase.adv), _lib.ptr(phase.coeffs), _lib.ptr(phase.stats), _lib.ptr(ws), ws.numel() * 8,
+                  _lib.stream())
     phase.adj_avg_rewards = None
     phase.invalidate_host()
 
 
-def _flat_paths_to_device(paths, dev):
-    """A flat list of (variable-length) host paths -> (obs [n,Do] float32, path_off [P+1] int32) on the device."""
-    import torch
-    lens = [len(p["observations"]) for p in paths]
-    obs = np.concatenate([np.asarray(p["observations"], dtype=np.float32).reshape(l, -1) for p, l in zip(paths, lens)])
+def _path_offsets(paths):
+    """Prefix sums [P+1] int32 of the path lengths len(path["observations"]) (the reference's time index restarts in every
+    path, baselines/linear_baseline.py:104, 124)."""
     off = np.zeros(len(paths) + 1, dtype=np.int32)
-    off[1:] = np.cumsum(lens)
+    off[1:] = np.cumsum([len(p["observations"]) for p in paths])
+    return off
+
+
+def _flat_paths_to_device(paths, dev, with_obs=True):
+    """A flat list of (variable-length) host paths -> (obs [n,Do] float32 or None, path_off [P+1] int32, n, Do) on the
+    device.  with_obs=False (LinearTimeBaseline): only the path table is uploaded, Do = 1."""
+    import torch
+    off = _path_offsets(paths)
+    if not with_obs:
+        return None, torch.from_numpy(off).to(dev), int(off[-1]), 1
+    obs = np.concatenate([np.asarray(p["observations"], dtype=np.float32).reshape(int(off[k + 1] - off[k]), -1)
+                          for k, p in enumerate(paths)])
     return (torch.from_numpy(np.ascontiguousarray(obs)).to(dev), torch.from_numpy(off).to(dev), int(off[-1]), obs.shape[1])
 
 
-def fit_baseline_on_paths(paths, target_key, reg_coeff):
+def fit_baseline_on_paths(paths, target_key, reg_coeff, kind=_lib.BASELINE_LINEAR_FEATURE):
     """LinearBaseline.fit (baselines/linear_baseline.py:55-77) on the device: float64 Gram matrix of the
-    LinearFeatureBaseline features + ridge solve with the reference's x10-on-NaN retry (promp_baseline_fit).
-    Returns the coefficient vector [2*Do+4] as a host float64 array."""
+    LinearFeatureBaseline (kind 1) or LinearTimeBaseline (kind 2) features + ridge solve with the reference's x10-on-NaN
+    retry (promp_baseline_fit_ex).  Returns the coefficient vector (2*Do+4 or 4) as a host float64 array."""
     import torch
     _lib.require_cuda()
     assert all(target_key in p.keys() for p in paths)
     dev = torch.device('cuda', torch.cuda.current_device())
-    obs, off, n, Do = _flat_paths_to_device(paths, dev)
+    obs, off, n, Do = _flat_paths_to_device(paths, dev, with_obs=kind == _lib.BASELINE_LINEAR_FEATURE)
     target = torch.from_numpy(np.concatenate([np.asarray(p[target_key], dtype=np.float64).reshape(-1) for p in paths])).to(dev)
     assert target.numel() == n, "targets and observations must have the same length"
-    coeffs = torch.empty(2 * Do + 4, dtype=torch.float64, device=dev)
+    coeffs = torch.empty(_coeff_width(kind, Do), dtype=torch.float64, device=dev)
     ws = _zeroed_workspace(_lib.load().promp_baseline_fit_workspace_bytes(len(paths), n, Do), dev)
-    _lib.call('promp_baseline_fit', len(paths), n, Do, _lib.ptr(obs), _lib.ptr(target), _lib.ptr(off), float(reg_coeff),
-              _lib.ptr(coeffs), None, _lib.ptr(ws), ws.numel() * 8, _lib.stream())
+    _lib.call('promp_baseline_fit_ex', int(kind), len(paths), n, Do, _lib.ptr(obs), _lib.ptr(target), _lib.ptr(off),
+              float(reg_coeff), _lib.ptr(coeffs), None, _lib.ptr(ws), ws.numel() * 8, _lib.stream())
     return coeffs.cpu().numpy()
 
 
-def predict_baseline_on_path(path, coeffs):
-    """LinearBaseline.predict (baselines/linear_baseline.py:17-33) on the device (promp_baseline_predict)."""
+def predict_baseline_on_path(path, coeffs, kind=_lib.BASELINE_LINEAR_FEATURE):
+    """LinearBaseline.predict (baselines/linear_baseline.py:17-33) on the device (promp_baseline_predict_ex)."""
     import torch
     _lib.require_cuda()
     dev = torch.device('cuda', torch.cuda.current_device())
-    obs, off, n, Do = _flat_paths_to_device([path], dev)
+    obs, off, n, Do = _flat_paths_to_device([path], dev, with_obs=kind == _lib.BASELINE_LINEAR_FEATURE)
     w = torch.from_numpy(np.ascontiguousarray(np.asarray(coeffs, dtype=np.float64))).to(dev)
-    assert w.numel() == 2 * Do + 4, "coefficient vector does not match the observation dimension"
+    assert w.numel() == _coeff_width(kind, Do), "coefficient vector does not match the baseline's features"
     out = torch.empty(n, dtype=torch.float64, device=dev)
-    _lib.call('promp_baseline_predict', 1, n, Do, _lib.ptr(obs), _lib.ptr(off), _lib.ptr(w), _lib.ptr(out), _lib.stream())
+    _lib.call('promp_baseline_predict_ex', int(kind), 1, n, Do, _lib.ptr(obs), _lib.ptr(off), _lib.ptr(w), _lib.ptr(out),
+              _lib.stream())
     return out.cpu().numpy()
+
+
+def _host_task_paths(phase, m):
+    """Task m of a processed phase as the reference's path dicts (meta_sampler.py:116-123) plus 'returns'
+    (samplers/base.py:103-104), from one host copy of the phase's tensors.  Arrays are float32, as the phase stores them."""
+    if isinstance(phase, RaggedPhaseData):
+        bounds = phase.path_off_host[m][:int(phase.n_paths_host[m]) + 1]
+    else:
+        bounds = np.arange(phase.E + 1) * phase.H
+    obs, act, rew, ret, mean = (phase.host(k)[m] for k in ('obs', 'act', 'rew', 'returns', 'mean'))
+    log_std = phase.host('log_std')[m]
+    info = phase.host('info') if phase.info_keys else None
+    paths = []
+    for k in range(len(bounds) - 1):
+        s = slice(int(bounds[k]), int(bounds[k + 1]))
+        paths.append(dict(observations=obs[s], actions=act[s], rewards=rew[s], returns=ret[s],
+                          env_infos={key: info[i, m, s] for i, key in enumerate(phase.info_keys)},
+                          agent_infos=dict(mean=mean[s], log_std=np.broadcast_to(log_std, (s.stop - s.start, phase.act_dim)))))
+    return paths
 
 
 class MetaSampleProcessor(object):
@@ -203,14 +258,43 @@ class MetaSampleProcessor(object):
         self.positive_adv = positive_adv
 
     def process_phase(self, phase):
-        """Device-only entry: run the processing kernel on a PhaseData (no host traffic)."""
+        """Run the processing kernel on a PhaseData.  With a device baseline (`device_kind`) nothing leaves the device;
+        any other baseline object goes through _process_phase_host_baseline."""
+        kind = _baseline_kind(self.baseline)
+        if kind is None:
+            return self._process_phase_host_baseline(phase)
         run_process_kernel(phase, self.discount, self.gae_lambda, getattr(self.baseline, '_reg_coeff', 1e-5),
-                           _baseline_kind(self.baseline), self.normalize_adv, self.positive_adv)
-        if hasattr(self.baseline, '_coeffs') and _baseline_kind(self.baseline) == 1:
+                           kind, self.normalize_adv, self.positive_adv)
+        if hasattr(self.baseline, '_coeffs') and kind in (_lib.BASELINE_LINEAR_FEATURE, _lib.BASELINE_LINEAR_TIME):
             # the reference's baseline object holds the last fit = the last task's (baselines/linear_baseline.py:55-77): a lazy
             # view of the device buffer, fetched on demand (a replayed CUDA graph rewrites the same buffer every iteration)
             self.baseline._lazy_coeffs = (phase, phase.M - 1)
             self.baseline._coeffs = _LazyCoeffs(phase)
+        return phase
+
+    def _process_phase_host_baseline(self, phase):
+        """A baseline with fit / predict but no device kind (samplers/base.py:99-108 asserts nothing more):
+          1. the ZERO kind computes the discounted returns on the device (the same returns the final pass writes);
+          2. for tasks m = 0..M-1 in order, the task's path dicts, 'returns' included, go to baseline.fit(paths,
+             target_key='returns'), then baseline.predict(path) runs for each path in order - the reference's sequence, so
+             the object is left fitted on the last task.  The arrays are float32 (observations, rewards and returns as
+             the phase stores them), not the reference's float64 returns;
+          3. every prediction goes up in one H2D copy and the GIVEN kind runs GAE, normalisation and the statistics."""
+        import torch
+        run_process_kernel(phase, self.discount, self.gae_lambda, 0.0, _lib.BASELINE_ZERO, self.normalize_adv,
+                           self.positive_adv)
+        values = np.zeros((phase.M, phase.N), dtype=np.float64)
+        for m in range(phase.M):
+            paths = _host_task_paths(phase, m)
+            self.baseline.fit(paths, target_key='returns')
+            n = 0
+            for p in paths:
+                L = len(p['rewards'])
+                values[m, n:n + L] = np.asarray(self.baseline.predict(p), dtype=np.float64).reshape(L)
+                n += L
+        given = torch.from_numpy(values).to(phase.obs.device)
+        run_process_kernel(phase, self.discount, self.gae_lambda, 0.0, _lib.BASELINE_GIVEN, self.normalize_adv,
+                           self.positive_adv, given=given)
         return phase
 
     def compute_adj_avg_rewards(self, phase, allreduce=None):

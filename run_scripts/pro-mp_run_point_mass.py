@@ -9,7 +9,7 @@ import sys
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from promp_b200.baselines import LinearFeatureBaseline  # noqa: E402,F401
+from promp_b200.baselines import LinearFeatureBaseline, LinearTimeBaseline  # noqa: E402,F401
 from promp_b200.envs import MetaPointEnvCorner, HalfCheetahRandDirecEnv, normalize  # noqa: E402,F401
 from promp_b200.meta_algos import ProMP  # noqa: E402
 from promp_b200.meta_trainer import Trainer  # noqa: E402
