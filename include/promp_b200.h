@@ -66,6 +66,11 @@ enum {
  * promp_num_params, promp_policy_layout and the workspace sizes do not depend on the activation. */
 #define PROMP_HIDDEN_WIDTH_MASK 0xFF
 #define PROMP_ACT_RELU 0x100
+/* Output non-linearity of the mean (policies/networks/mlp.py: output_nonlinearity), in the same `hidden` argument: no flag =
+ * identity, PROMP_OUT_TANH = mean = tanh(h2 W2 + b2).  It combines with either hidden activation (width | PROMP_ACT_RELU |
+ * PROMP_OUT_TANH), at width 32 or 64, and does not change the layout or the workspace sizes either.  Bits 0x200 - 0x800
+ * stay unknown (rejected). */
+#define PROMP_OUT_TANH 0x1000
 /* baseline kinds of promp_process_samples.  LINEAR_TIME (baselines/linear_baseline.py:109-126) fits [t, t^2, t^3, 1],
  * t = step / 100, and never reads obs; its coefficients are [M,4].  GIVEN: the caller supplies the per-sample baseline
  * values (promp_process_samples_given); no fit, no coefficients. */

@@ -11,7 +11,8 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(ROOT, 'build', 'obj')
 LIB = os.path.join(PKG, 'libpromp_b200.so')
-SOURCES = ('common.cu', 'rollout.cu', 'process.cu', 'policy.cu', 'policy_relu.cu', 'comm.cu', 'trpo.cu', 'paths.cu')
+SOURCES = ('common.cu', 'rollout.cu', 'process.cu', 'policy.cu', 'policy_relu.cu', 'policy_otanh.cu', 'policy_relu_otanh.cu', 'comm.cu',
+           'trpo.cu', 'paths.cu')
 NVCC_FLAGS = ['-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 

@@ -19,8 +19,8 @@ INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE, OBJ_EXPLORE = 0, 1, 2, 3, 4
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE, BASELINE_LINEAR_TIME, BASELINE_GIVEN = 0, 1, 2, 3
-# the policy / rollout `hidden` argument: width | activation flag (no flag = tanh)
-HIDDEN_WIDTH_MASK, ACT_RELU = 0xFF, 0x100
+# the policy / rollout `hidden` argument: width | activation flag (no flag = tanh) | output flag (no flag = identity)
+HIDDEN_WIDTH_MASK, ACT_RELU, OUT_TANH = 0xFF, 0x100, 0x1000
 
 _P = c_void_p
 

@@ -23,7 +23,8 @@ int check_cuda(cudaError_t e, const char* what) {
 extern "C" const char* promp_last_error(void) { return promp::g_err; }
 extern "C" int promp_version(void) { return 100; }
 extern "C" int promp_num_params(int obs_dim, int act_dim, int hidden) {
-    // the activation does not change the layout: (32 | 64) | PROMP_ACT_RELU count as their width
-    if (hidden == (32 | PROMP_ACT_RELU) || hidden == (64 | PROMP_ACT_RELU)) hidden &= PROMP_HIDDEN_WIDTH_MASK;
+    // the activations do not change the layout: (32 | 64) with PROMP_ACT_RELU and / or PROMP_OUT_TANH count as their width
+    const int width = hidden & PROMP_HIDDEN_WIDTH_MASK, flags = hidden & ~PROMP_HIDDEN_WIDTH_MASK;
+    if ((width == 32 || width == 64) && flags != 0 && (flags & ~(PROMP_ACT_RELU | PROMP_OUT_TANH)) == 0) hidden = width;
     return promp::num_params(obs_dim, act_dim, hidden);
 }

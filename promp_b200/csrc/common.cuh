@@ -78,8 +78,10 @@ __device__ __forceinline__ float tanh_fast(float x) {
 //              second-derivative term sigma''(z) * zdot is dd_d(h) * r (tanh: -2 h r).
 // CURVED = false says sigma'' = 0 everywhere the kernels evaluate it (ReLU): the Hessian-vector kernels drop the
 // second-derivative terms at compile time.
+// OUT_TANH = false: the trait's policy has the identity output layer (see OutTanh below).
 struct ActTanh {
     static constexpr bool CURVED = true;
+    static constexpr bool OUT_TANH = false;
     __device__ __forceinline__ static float f(float z) { return tanh_fast(z); }
     __device__ __forceinline__ static float d(float h) { return 1.f - h * h; }
     __device__ __forceinline__ static float dd_d(float h) { return -2.f * h; }
@@ -87,8 +89,17 @@ struct ActTanh {
 // sigma'(0) = 0, as TensorFlow's ReluGrad (the gradient flows only where the output is positive)
 struct ActRelu {
     static constexpr bool CURVED = false;
+    static constexpr bool OUT_TANH = false;
     __device__ __forceinline__ static float f(float z) { return fmaxf(z, 0.f); }
     __device__ __forceinline__ static float d(float h) { return h > 0.f ? 1.f : 0.f; }
+};
+// The same hidden activation with a tanh output layer: mean = tanh(h2 W2 + b2) (policies/networks/mlp.py:53-56, 93-113,
+// output_nonlinearity=tf.tanh).  The policy kernels take the pair as their one activation parameter; the out_* helpers
+// below are no-ops for the identity output, so the kernels of ActTanh / ActRelu keep their code.
+template <class Hid>
+struct OutTanh : Hid {
+    using Hidden = Hid;
+    static constexpr bool OUT_TANH = true;
 };
 
 // Backward step of the Hessian-vector product through one hidden layer:  c * sigma'(z) + ac * dh * sigma''(z) * zdot,
@@ -99,15 +110,60 @@ __device__ __forceinline__ float act_hvp_back(float c, float dh, float h, float 
     else return c * Act::d(h);
 }
 
-// The `hidden` argument of the policy and rollout entry points: the width (32 or 64) in the low byte, PROMP_ACT_* flags
-// above it.  A plain width selects tanh.
-inline int decode_hidden(const char* who, int hidden, int& width, bool& relu) {
-    PROMP_REQUIRE((hidden & ~(PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU)) == 0,
-                  "%s: unknown flag bits 0x%x in hidden (%d); known: PROMP_ACT_RELU = 0x%x", who,
-                  hidden & ~(PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU), hidden, PROMP_ACT_RELU);
+// ---- output layer of the mean, for DA action dimensions.  mu holds z = h2 W2 + b2 on entry, the mean on exit.
+template <class Act, int DA>
+__device__ __forceinline__ void out_forward(float (&mu)[DA]) {
+    if constexpr (Act::OUT_TANH) {
+#pragma unroll
+        for (int d = 0; d < DA; ++d) mu[d] = ActTanh::f(mu[d]);
+    }
+}
+// ... and the tangent: rmu holds zdot on entry, the mean's tangent (1 - mu^2) zdot on exit
+template <class Act, int DA>
+__device__ __forceinline__ void out_forward_tangent(float (&mu)[DA], float (&rmu)[DA]) {
+    if constexpr (Act::OUT_TANH) {
+#pragma unroll
+        for (int d = 0; d < DA; ++d) {
+            mu[d] = ActTanh::f(mu[d]);
+            rmu[d] *= ActTanh::d(mu[d]);
+        }
+    }
+}
+// Gradient: the head's d loss / d mu -> d loss / d z
+template <class Act, int DA>
+__device__ __forceinline__ void out_grad_back(const float (&mu)[DA], float (&dmu)[DA]) {
+    if constexpr (Act::OUT_TANH) {
+#pragma unroll
+        for (int d = 0; d < DA; ++d) dmu[d] *= ActTanh::d(mu[d]);
+    }
+}
+// Hessian-vector product: the head's signals at mu (dmu, cmu; rmu = the mean's tangent) -> their values at z.  The same
+// step as a hidden layer's (act_hvp_back), with the mean in place of h:  C_z = (1 - mu^2) cmu + ac dmu (-2 mu) rmu.
+template <class Act, int DA>
+__device__ __forceinline__ void out_hvp_back(const float (&mu)[DA], const float (&rmu)[DA], float ac, float (&dmu)[DA],
+                                             float (&cmu)[DA]) {
+    if constexpr (Act::OUT_TANH) {
+#pragma unroll
+        for (int d = 0; d < DA; ++d) {
+            cmu[d] = act_hvp_back<ActTanh>(cmu[d], dmu[d], mu[d], rmu[d], ac);
+            dmu[d] *= ActTanh::d(mu[d]);
+        }
+    }
+}
+
+// The `hidden` argument of the policy and rollout entry points: the width (32 or 64) in the low byte, PROMP_ACT_RELU and
+// PROMP_OUT_TANH above it.  A plain width selects tanh hidden layers and the identity output.
+inline int decode_hidden(const char* who, int hidden, int& width, bool& relu, bool& out_tanh) {
+    constexpr int known = PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU | PROMP_OUT_TANH;
+    PROMP_REQUIRE((hidden & ~known) == 0,
+                  "%s: unknown flag bits 0x%x in hidden (%d); known: PROMP_ACT_RELU = 0x%x, PROMP_OUT_TANH = 0x%x", who,
+                  hidden & ~known, hidden, PROMP_ACT_RELU, PROMP_OUT_TANH);
     width = hidden & PROMP_HIDDEN_WIDTH_MASK;
     relu = (hidden & PROMP_ACT_RELU) != 0;
+    out_tanh = (hidden & PROMP_OUT_TANH) != 0;
     PROMP_REQUIRE(!relu || width == 32 || width == 64, "%s: ReLU policies are built for hidden 32 or 64 (got %d)", who, width);
+    PROMP_REQUIRE(!out_tanh || width == 32 || width == 64, "%s: tanh-output policies are built for hidden 32 or 64 (got %d)",
+                  who, width);
     return PROMP_OK;
 }
 

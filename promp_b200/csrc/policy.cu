@@ -16,8 +16,19 @@
 // This file is compiled twice: as itself (tanh: every kernel, option, entry point) and through policy_relu.cu, which
 // defines PROMP_POLICY_RELU_TU and compiles only the ReLU instantiations of the templated kernels and launchers
 // (namespace promp::relu_tu below).  Separate translation units keep the tanh kernels' code exactly what it was before
-// ReLU existed, and the two halves compile in parallel.
-#ifdef PROMP_POLICY_RELU_TU
+// ReLU existed, and the two halves compile in parallel.  The tanh-output policies (OutTanh<ActTanh>, OutTanh<ActRelu>) are two
+// more units of the same kind: policy_otanh.cu (PROMP_POLICY_OTANH_TU, namespace otanh_tu) and policy_relu_otanh.cu (both
+// macros, namespace relu_otanh_tu).  PROMP_POLICY_EXTRA_TU marks every unit but this one.
+#if defined(PROMP_POLICY_RELU_TU) || defined(PROMP_POLICY_OTANH_TU)
+#define PROMP_POLICY_EXTRA_TU
+#endif
+#if defined(PROMP_POLICY_RELU_TU) && defined(PROMP_POLICY_OTANH_TU)
+#define PROMP_POLICY_ACT OutTanh<ActRelu>
+#define PROMP_ACT_NS relu_otanh_tu
+#elif defined(PROMP_POLICY_OTANH_TU)
+#define PROMP_POLICY_ACT OutTanh<ActTanh>
+#define PROMP_ACT_NS otanh_tu
+#elif defined(PROMP_POLICY_RELU_TU)
 #define PROMP_POLICY_ACT ActRelu
 #define PROMP_ACT_NS relu_tu
 #else
@@ -229,8 +240,10 @@ __device__ __forceinline__ void policy_grad_body(const PolicyArgs& A) {
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
+                    out_forward<Act, DA>(mu);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                     grad_signal<DA>(hin, o, A.obj_scale, kl_eff, invN, dmu, dls);
+                    out_grad_back<Act, DA>(mu, dmu);
                     s_obj += o.obj;
                     s_kl += o.kl;
                     s_ratio += o.ratio;
@@ -324,6 +337,15 @@ __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_explore_kernel(Poli
 template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_explore_relu_kernel(PolicyArgs A) {
     policy_grad_body<DO, DA, HID, ActRelu, ADV_TASK>(A);
+}
+// tanh output layer: *_otanh_kernel<..., Hid> for hidden activation Hid (ActTanh or ActRelu)
+template <int DO, int DA, int HID, class Hid>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_otanh_kernel(PolicyArgs A) {
+    policy_grad_body<DO, DA, HID, OutTanh<Hid>>(A);
+}
+template <int DO, int DA, int HID, class Hid>
+__global__ void __launch_bounds__(PT_THREADS, 2) policy_grad_explore_otanh_kernel(PolicyArgs A) {
+    policy_grad_body<DO, DA, HID, OutTanh<Hid>, ADV_TASK>(A);
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -557,8 +579,10 @@ __device__ __forceinline__ void policy_hvp_body(const PolicyArgs& A) {
                     HeadOut<DA> o;
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
+                    out_forward_tangent<Act, DA>(mu, rmu);
                     gaussian_head<DA>(hin, ho, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                     hvp_signal<DA>(hin, o, rmu, rls, A.obj_kind, kl_eff, invN, ac, dA, dmu, cmu, cls);
+                    out_hvp_back<Act, DA>(mu, rmu, ac, dmu, cmu);
                     s_obj += o.obj;
                     s_kl += o.kl;
                     s_ratio += o.ratio;
@@ -668,6 +692,8 @@ template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS) policy_hvp_kernel(PolicyArgs A) { policy_hvp_body<DO, DA, HID, ActTanh>(A); }
 template <int DO, int DA, int HID>
 __global__ void __launch_bounds__(PT_THREADS) policy_hvp_relu_kernel(PolicyArgs A) { policy_hvp_body<DO, DA, HID, ActRelu>(A); }
+template <int DO, int DA, int HID, class Hid>
+__global__ void __launch_bounds__(PT_THREADS) policy_hvp_otanh_kernel(PolicyArgs A) { policy_hvp_body<DO, DA, HID, OutTanh<Hid>>(A); }
 
 // -------------------------------------------------------------------------------------------------
 // forward only: mean for arbitrary obs (distribution_info_sym / get_actions without sampling).  obs_dim / act_dim: the
@@ -709,7 +735,8 @@ __device__ __forceinline__ void policy_forward_body(int M, int N, const float* p
         }
 #pragma unroll
         for (int d = 0; d < DA; ++d) {
-            const float s = warp_sum(mu[d]) + sP[L::B2 + d];
+            float s = warp_sum(mu[d]) + sP[L::B2 + d];
+            if constexpr (Act::OUT_TANH) s = ActTanh::f(s);
             if (lane == d && d < dA) mean[((int64_t)m * N + n) * dA + d] = s;
         }
         __syncwarp();
@@ -726,8 +753,13 @@ __global__ void __launch_bounds__(128) policy_forward_relu_kernel(int M, int N, 
                                                                    const float* obs, float* mean, int obs_dim, int act_dim) {
     policy_forward_body<DO, DA, HID, ActRelu>(M, N, params, stride, obs, mean, obs_dim, act_dim);
 }
+template <int DO, int DA, int HID, class Hid>
+__global__ void __launch_bounds__(128) policy_forward_otanh_kernel(int M, int N, const float* params, int64_t stride,
+                                                                    const float* obs, float* mean, int obs_dim, int act_dim) {
+    policy_forward_body<DO, DA, HID, OutTanh<Hid>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
+}
 
-#ifndef PROMP_POLICY_RELU_TU
+#ifndef PROMP_POLICY_EXTRA_TU
 __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, float* out) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P) return;
@@ -871,11 +903,11 @@ __global__ void adapt_kl_coeff_kernel(int S1, const float* __restrict__ final_te
     }
 }
 
-#endif  // !PROMP_POLICY_RELU_TU
+#endif  // !PROMP_POLICY_EXTRA_TU
 
 // -------------------------------------------------------------------------------------------------
 // options of promp_set_option, defined by the tanh translation unit and read by both
-#ifdef PROMP_POLICY_RELU_TU
+#ifdef PROMP_POLICY_EXTRA_TU
 #define PROMP_OPTION(name, init) extern int name
 #else
 #define PROMP_OPTION(name, init) int name = init
@@ -947,9 +979,11 @@ static int launch_policy(Kernel kernel, int smem, int& occ_cache, PolicyArgs& A,
 // names only the selected one, so a tanh launcher instantiates exactly the kernels it did before ReLU existed.
 template <class Act>
 constexpr bool is_relu() { return std::is_same<Act, ActRelu>::value; }
+// A tanh output layer selects policy_*_otanh_kernel<..., hidden activation>.
 #define PROMP_ACT_KERNEL(Act, NAME, ...)                                                               \
     [] {                                                                                               \
-        if constexpr (is_relu<Act>()) return NAME##_relu_kernel<__VA_ARGS__>;                          \
+        if constexpr (Act::OUT_TANH) return NAME##_otanh_kernel<__VA_ARGS__, typename Act::Hidden>;    \
+        else if constexpr (is_relu<Act>()) return NAME##_relu_kernel<__VA_ARGS__>;                     \
         else return NAME##_kernel<__VA_ARGS__>;                                                        \
     }()
 
@@ -1228,7 +1262,8 @@ static int launch_forward(int M, int N, const float* params, int64_t stride, con
     }
 
 // The (obs, act, hidden) dispatch of every entry point for this translation unit's activation: tanh_tu:: here, relu_tu:: in
-// policy_relu.cu.  `hidden` has been checked by decode_hidden; padded = the bucket table of the *_padded entry points.
+// policy_relu.cu, otanh_tu:: and relu_otanh_tu:: in the tanh-output units.  `hidden` has been checked by decode_hidden;
+// padded = the bucket table of the *_padded entry points.
 namespace PROMP_ACT_NS {
 #define PROMP_DISPATCH(FN, ...)                                                  \
     const int hid_ = hidden & PROMP_HIDDEN_WIDTH_MASK;                          \
@@ -1257,29 +1292,36 @@ int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, con
 }
 }  // namespace PROMP_ACT_NS
 
-#ifndef PROMP_POLICY_RELU_TU
-namespace relu_tu {      // policy_relu.cu
-int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);
-int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);
-int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns,
-                              int M);
-int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M);
-int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag,
-          const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);
-int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride, const float* obs,
-            float* mean, cudaStream_t s);
-}  // namespace relu_tu
+#ifndef PROMP_POLICY_EXTRA_TU
+// the dispatch of the other units: relu_tu (policy_relu.cu), otanh_tu (policy_otanh.cu), relu_otanh_tu (policy_relu_otanh.cu)
+#define PROMP_DECLARE_UNIT(NS)                                                                                                    \
+    namespace NS {                                                                                                                \
+    int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);       \
+    int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);        \
+    int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds,              \
+                                  const int* Ns, int M);                                                                          \
+    int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M);  \
+    int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A,                   \
+              const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);                         \
+    int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride,             \
+                const float* obs, float* mean, cudaStream_t s);                                                                   \
+    }
+PROMP_DECLARE_UNIT(relu_tu)
+PROMP_DECLARE_UNIT(otanh_tu)
+PROMP_DECLARE_UNIT(relu_otanh_tu)
 #endif
 
-// checks `hidden` (decode_hidden) and selects the dispatch namespace of its activation; returns from the caller on bad bits
+// checks `hidden` (decode_hidden) and decodes its activations; returns from the caller on bad bits
 #define PROMP_DECODE_HIDDEN(who)                                                                 \
     int hid_ = 0;                                                                                \
-    bool relu_ = false;                                                                          \
-    if (decode_hidden(who, hidden, hid_, relu_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    bool relu_ = false, otanh_ = false;                                                          \
+    if (decode_hidden(who, hidden, hid_, relu_, otanh_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+// dispatch function FN of the unit that holds the decoded activations' kernels
+#define PROMP_UNIT(FN) (otanh_ ? (relu_ ? relu_otanh_tu::FN : otanh_tu::FN) : (relu_ ? relu_tu::FN : tanh_tu::FN))
 
 }  // namespace promp
 
-#ifndef PROMP_POLICY_RELU_TU
+#ifndef PROMP_POLICY_EXTRA_TU
 
 using namespace promp;
 
@@ -1299,9 +1341,9 @@ extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int a
 
 extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]) {
     PROMP_REQUIRE(out != nullptr, "promp_policy_layout: null output");
-    int width;           // the activation does not change the layout
-    bool relu;
-    if (decode_hidden("promp_policy_layout", hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    int width;           // the activations do not change the layout
+    bool relu, out_tanh;
+    if (decode_hidden("promp_policy_layout", hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     hidden = width;
     PROMP_REQUIRE(obs_dim >= 1 && obs_dim <= 19 && act_dim >= 1 && act_dim <= 8 && (hidden == 32 || hidden == 64),
                   "promp_policy_layout: padded policy kernels take obs_dim in [1, 19], act_dim in [1, 8] and hidden 32 or 64 "
@@ -1360,7 +1402,7 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
     explore_args(A);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_grad")
-    return (relu_ ? relu_tu::grad : tanh_tu::grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
+    return PROMP_UNIT(grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_GRAD_EX_PARAMS                                                                                               \
@@ -1419,7 +1461,7 @@ static int policy_hvp_impl(bool padded, int obs_dim, int act_dim, int hidden, in
     A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_hvp")
-    return (relu_ ? relu_tu::hvp : tanh_tu::hvp)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
+    return PROMP_UNIT(hvp)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_HVP_RAGGED_PARAMS                                                                                            \
@@ -1486,8 +1528,7 @@ static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int a
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_workspace_bytes")
-    return (relu_ ? relu_tu::chain_workspace_bytes : tanh_tu::chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, n_stages,
-                                                                                      kinds, Ns, M);
+    return PROMP_UNIT(chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
 }
 extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                       const promp_policy_stage* stages) {
@@ -1504,7 +1545,7 @@ static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim,
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_num_launches")
-    return (relu_ ? relu_tu::chain_launches : tanh_tu::chain_launches)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
+    return PROMP_UNIT(chain_launches)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
 }
 extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                const promp_policy_stage* stages) {
@@ -1529,8 +1570,8 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
     for (int k = 0; k < n_stages; ++k) A[k].obs_dim = obs_dim, A[k].act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_chain")
-    return (relu_ ? relu_tu::chain : tanh_tu::chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta,
-                                                    workspace, workspace_bytes, s);
+    return PROMP_UNIT(chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta, workspace,
+                             workspace_bytes, s);
 }
 extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
                                   const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
@@ -1579,7 +1620,7 @@ static int policy_forward_impl(bool padded, int obs_dim, int act_dim, int hidden
     PROMP_REQUIRE(M <= 65535, "promp_policy_forward: M=%d exceeds the grid.y limit", M);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_forward")
-    return (relu_ ? relu_tu::forward : tanh_tu::forward)(padded, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, s);
+    return PROMP_UNIT(forward)(padded, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, s);
 }
 extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
                                     int64_t param_stride, const float* obs, float* mean, void* stream) {
@@ -1667,4 +1708,4 @@ extern "C" int promp_debug_phase_clocks(unsigned long long* out16, int reset) {
     return 0;
 }
 #endif
-#endif  // !PROMP_POLICY_RELU_TU
+#endif  // !PROMP_POLICY_EXTRA_TU

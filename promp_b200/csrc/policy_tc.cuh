@@ -558,6 +558,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     adv = load_head_sample<DA, ADV>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
                 }
                 HeadOut<DA> o;
+                out_forward<Act, DA>(mu);
                 if (A.ls_per_sample) {
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
@@ -566,6 +567,7 @@ __device__ __forceinline__ void grad_tc_tiles(const PolicyArgs& A, GradTcSmem<DO
                     gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
                 grad_signal<DA>(hin, o, A.obj_scale, kl_eff, invN, dmu, dls);
+                out_grad_back<Act, DA>(mu, dmu);
                 s_obj += o.obj;
                 s_kl += o.kl;
                 s_ratio += o.ratio;
@@ -695,6 +697,15 @@ __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_explore_kernel(Pol
 template <int DO, int DA, int NQ>
 __global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_explore_relu_kernel(PolicyArgs A) {
     policy_grad_tc_body<DO, DA, NQ, ActRelu, ADV_TASK>(A);
+}
+// tanh output layer, for hidden activation Hid
+template <int DO, int DA, int NQ, class Hid>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_otanh_kernel(PolicyArgs A) {
+    policy_grad_tc_body<DO, DA, NQ, OutTanh<Hid>>(A);
+}
+template <int DO, int DA, int NQ, class Hid>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_grad_tc_explore_otanh_kernel(PolicyArgs A) {
+    policy_grad_tc_body<DO, DA, NQ, OutTanh<Hid>, ADV_TASK>(A);
 }
 
 
@@ -1010,6 +1021,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                     adv = load_head_sample<DA>(A, g0 + r, m, dA, A.ls_per_sample, a, mo, lso);
                 }
                 HeadOut<DA> o;
+                out_forward_tangent<Act, DA>(mu, rmu);
                 if (A.ls_per_sample) {
                     HeadOld<DA> ho;
                     head_old_from<DA>(lso, ho, dA);
@@ -1018,6 +1030,7 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
                     gaussian_head<DA>(hin, S.hold, mu, a, mo, adv, A.obj_kind, A.clip_eps, o, dA);
                 }
                 hvp_signal<DA>(hin, o, rmu, rls, A.obj_kind, kl_eff, invN, ac, dA, dmu, cmu, cls);
+                out_hvp_back<Act, DA>(mu, rmu, ac, dmu, cmu);
                 s_obj += o.obj;
                 s_kl += o.kl;
                 s_ratio += o.ratio;
@@ -1152,6 +1165,10 @@ template <int DO, int DA, int NQ>
 __global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_kernel(PolicyArgs A) { policy_hvp_tc_body<DO, DA, NQ, ActTanh>(A); }
 template <int DO, int DA, int NQ>
 __global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_relu_kernel(PolicyArgs A) { policy_hvp_tc_body<DO, DA, NQ, ActRelu>(A); }
+template <int DO, int DA, int NQ, class Hid>
+__global__ void __launch_bounds__(128 * NQ, 1) policy_hvp_tc_otanh_kernel(PolicyArgs A) {
+    policy_hvp_tc_body<DO, DA, NQ, OutTanh<Hid>>(A);
+}
 
 // =================================================================================================================
 // Dataflow kernel: the whole gradient chain of one meta-objective evaluation in ONE persistent launch
@@ -1196,10 +1213,17 @@ struct ChainSmem {
     static constexpr int SIZE = BODY + 16;     // + current item
 };
 
-// One chain kernel per translation unit (policy.cu / policy_relu.cu), for that unit's activation: policy_chain_tc_kernel
-// (tanh) or policy_chain_tc_relu_kernel (ReLU).  The body is written in the kernel itself: passed on to a device function
-// by reference, the __grid_constant__ argument changed the tanh kernels' code.
-#ifdef PROMP_POLICY_RELU_TU
+// One chain kernel per translation unit (policy.cu / policy_relu.cu / policy_otanh.cu / policy_relu_otanh.cu), for that unit's
+// activation: policy_chain_tc_kernel (tanh), policy_chain_tc_relu_kernel (ReLU), policy_chain_tc_otanh_kernel (tanh, tanh
+// output) or policy_chain_tc_relu_otanh_kernel (ReLU, tanh output).  The body is written in the kernel itself: passed on to a
+// device function by reference, the __grid_constant__ argument changed the tanh kernels' code.
+#if defined(PROMP_POLICY_RELU_TU) && defined(PROMP_POLICY_OTANH_TU)
+#define PROMP_CHAIN_KERNEL policy_chain_tc_relu_otanh_kernel
+using ChainAct = OutTanh<ActRelu>;
+#elif defined(PROMP_POLICY_OTANH_TU)
+#define PROMP_CHAIN_KERNEL policy_chain_tc_otanh_kernel
+using ChainAct = OutTanh<ActTanh>;
+#elif defined(PROMP_POLICY_RELU_TU)
 #define PROMP_CHAIN_KERNEL policy_chain_tc_relu_kernel
 using ChainAct = ActRelu;
 #else

@@ -213,6 +213,7 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
             }
 #pragma unroll
             for (int d = 0; d < DA; ++d) mu[d] = warp_sum(mu[d]) + b2[d];
+            out_forward<Act, DA>(mu);      // tanh output layer: mean = tanh(h2 W2 + b2)
 
             RCLK(4);
             // ---- sample: a = mean + eps * exp(log_std)      (gaussian_mlp_policy.py:74)
@@ -344,14 +345,25 @@ static int with_env(const char* fn, int env_kind, F&& f) {
     return PROMP_ERR_INVALID_ARG;
 }
 
-// `hidden` as decode_hidden gives it: width 32 or 64, ReLU or tanh
-static int launch_rollout(const char* fn, int env_kind, int width, bool relu, const RolloutArgs& A, cudaStream_t st) {
+// `hidden` as decode_hidden gives it: width 32 or 64, ReLU or tanh, identity or tanh output
+static int launch_rollout(const char* fn, int env_kind, int width, bool relu, bool out_tanh, const RolloutArgs& A,
+                          cudaStream_t st) {
     const dim3 grid((A.E + RO_WARPS - 1) / RO_WARPS, A.M);
     return with_env(fn, env_kind, [&](auto env) -> int {
         using Env = typename decltype(env)::type;
         const auto go = [&](auto keyed) {
             constexpr bool K = decltype(keyed)::value;
-            if (relu) {
+            if (out_tanh) {
+                using OR = OutTanh<ActRelu>;
+                using OT = OutTanh<ActTanh>;
+                if (relu) {
+                    if (width == 64) rollout_kernel<Env, 64, OR, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                    else rollout_kernel<Env, 32, OR, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                } else {
+                    if (width == 64) rollout_kernel<Env, 64, OT, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                    else rollout_kernel<Env, 32, OT, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
+                }
+            } else if (relu) {
                 if (width == 64) rollout_kernel<Env, 64, ActRelu, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
                 else rollout_kernel<Env, 32, ActRelu, K><<<grid, RO_WARPS * 32, 0, st>>>(A);
             } else {
@@ -396,8 +408,8 @@ static int rollout_fixed(const char* fn, int env_kind, int reward_type, float sp
     if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
     int width;
-    bool relu;
-    if (decode_hidden(fn, hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    bool relu, out_tanh;
+    if (decode_hidden(fn, hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
     PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "%s: bad reward_type %d", fn, reward_type);
     PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || info != nullptr,
@@ -413,7 +425,7 @@ static int rollout_fixed(const char* fn, int env_kind, int reward_type, float sp
     RolloutArgs A{reward_type, sparse_radius, normalize_actions, M, E, H, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, info, log_std_out,
                   final_state, 0, H, (uint32_t)task_offset * (uint32_t)E};
-    return launch_rollout(fn, env_kind, width, relu, A, (cudaStream_t)stream);
+    return launch_rollout(fn, env_kind, width, relu, out_tanh, A, (cudaStream_t)stream);
 }
 
 extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius, int normalize_actions, int M, int E, int H,
@@ -454,13 +466,13 @@ static int rollout_early_term(const char* fn, int env_kind, int normalize_action
     if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
     int width;
-    bool relu;
-    if (decode_hidden(fn, hidden, width, relu) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    bool relu, out_tanh;
+    if (decode_hidden(fn, hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
     RolloutArgs A{0, 0.f, normalize_actions, M, E, timeline_len, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
                   nullptr, 1, horizon, (uint32_t)task_offset * (uint32_t)E};
-    return launch_rollout(fn, env_kind, width, relu, A, (cudaStream_t)stream);
+    return launch_rollout(fn, env_kind, width, relu, out_tanh, A, (cudaStream_t)stream);
 }
 
 extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon, int hidden,

@@ -33,6 +33,15 @@ def _activation_name(fn):
     return name if name in ('tanh', 'relu') else None
 
 
+def _output_activation_name(fn):
+    """None (identity) or 'tanh' for a supported output_nonlinearity (None, 'tanh', or a callable named tanh such as tf.tanh /
+    torch.tanh); anything else is unsupported and returns False."""
+    if fn is None:
+        return None
+    name = fn if isinstance(fn, str) else getattr(fn, '__name__', None)
+    return 'tanh' if name == 'tanh' else False
+
+
 class MetaGaussianMLPPolicy(object):
     def __init__(self, meta_batch_size, obs_dim, action_dim, name='policy', hidden_sizes=(32, 32), learn_std=True,
                  hidden_nonlinearity='tanh', output_nonlinearity=None, init_std=1., min_std=1e-6, device=None,
@@ -47,8 +56,9 @@ class MetaGaussianMLPPolicy(object):
             raise NotImplementedError("promp_b200 policy kernels take obs_dim in [1, %d] and action_dim in [1, %d] (got %d, %d)"
                                       % (MAX_OBS_DIM, MAX_ACTION_DIM, int(obs_dim), int(action_dim)))
         act = _activation_name(hidden_nonlinearity)
-        if act is None or output_nonlinearity is not None:
-            raise NotImplementedError("promp_b200 kernels implement tanh or relu hidden / identity output non-linearities "
+        out = _output_activation_name(output_nonlinearity)
+        if act is None or out is False:
+            raise NotImplementedError("promp_b200 kernels implement tanh or relu hidden / identity or tanh output non-linearities "
                                       "(got hidden_nonlinearity=%r, output_nonlinearity=%r)"
                                       % (hidden_nonlinearity, output_nonlinearity))
         if not learn_std:
@@ -56,7 +66,7 @@ class MetaGaussianMLPPolicy(object):
                                       "the log_std variable to be trainable, gaussian_mlp_policy.py:174)")
         self._init_args = dict(meta_batch_size=meta_batch_size, obs_dim=int(obs_dim), action_dim=int(action_dim),
                                name=name, hidden_sizes=hidden_sizes, learn_std=learn_std, init_std=init_std,
-                               min_std=min_std, hidden_nonlinearity=act)
+                               min_std=min_std, hidden_nonlinearity=act, output_nonlinearity=out)
         self.meta_batch_size = meta_batch_size
         self.obs_dim, self.action_dim, self.name = int(obs_dim), int(action_dim), name
         # The kernels are instantiated for 32 and 64 hidden units; other widths run zero-padded: a padded unit has
@@ -64,8 +74,10 @@ class MetaGaussianMLPPolicy(object):
         # Hessian-vector product), and therefore stays zero under SGD / Adam / TRPO steps.
         self.hidden_sizes, self.hidden = hidden_sizes, (32 if max(hidden_sizes) <= 32 else 64)
         self.hidden_nonlinearity = act
-        # the `hidden` argument of every policy / rollout kernel call: the width, plus the activation flag for ReLU
-        self.hidden_arg = self.hidden | (_lib.ACT_RELU if act == 'relu' else 0)
+        self.output_nonlinearity = out        # None (identity) or 'tanh'
+        # the `hidden` argument of every policy / rollout kernel call: the width, plus the activation flag for ReLU and the
+        # output flag for a tanh mean
+        self.hidden_arg = self.hidden | (_lib.ACT_RELU if act == 'relu' else 0) | (_lib.OUT_TANH if out == 'tanh' else 0)
         self.learn_std = learn_std
         self.min_log_std = math.log(min_std)
         self.init_log_std = math.log(init_std)
@@ -251,6 +263,7 @@ class MetaGaussianMLPPolicy(object):
         return {'init_args': dict(self._init_args), 'network_params': self.get_param_values()}
 
     def __setstate__(self, state):
-        # no Xavier draw: loading must not consume np.random; a state saved before the activation was stored is tanh
+        # no Xavier draw: loading must not consume np.random; a state saved before the activations were stored is tanh with
+        # the identity output
         self.__init__(_skip_param_init=True, **state['init_args'])
         self.set_params(state['network_params'])

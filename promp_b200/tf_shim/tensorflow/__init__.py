@@ -46,7 +46,7 @@ def set_random_seed(seed):
     pass
 
 
-def tanh(x):            # lets run scripts keep passing hidden_nonlinearity=tf.tanh
+def tanh(x):            # lets run scripts pass hidden_nonlinearity=tf.tanh and output_nonlinearity=tf.tanh
     raise NotImplementedError("symbolic placeholder: promp_b200 policies evaluate tanh in CUDA")
 
 

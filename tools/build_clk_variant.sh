@@ -3,7 +3,7 @@
 set -e
 cd "$(dirname "$0")/.."
 mkdir -p build/obj_clk
-for f in common rollout process policy policy_relu comm trpo paths; do
+for f in common rollout process policy policy_relu policy_otanh policy_relu_otanh comm trpo paths; do
   nvcc -std=c++17 -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -Xcompiler -fPIC -DPROMP_EXP_CLOCKS -c promp_b200/csrc/$f.cu -o build/obj_clk/$f.o &
 done
 wait
