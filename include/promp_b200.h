@@ -487,7 +487,10 @@ int promp_policy_grad_ex(int obs_dim, int act_dim, int hidden, int M, int N, con
  * stage 0, as in promp_policy_grad_ex.  Shapes without tensor-core kernels (hidden != 64) and promp_set_option("chain", 0)
  * run the stages as separate launches.  The workspace (>= promp_policy_chain_workspace_bytes) starts with control words
  * that must be zero before the first call and are left zero: allocate it zero-filled once and do not share it with other
- * entry points.  `stages` is a HOST array (read during the call).
+ * entry points.  A call whose M differs from the previous call's on the same workspace clears the control words on the
+ * stream first, so one workspace serves chains of any M and stage count, on either path (the record of the last M is kept
+ * on the host: a workspace a captured CUDA graph uses is not used with another M outside that graph).  `stages` is a HOST
+ * array (read during the call).
  */
 typedef struct {
     int32_t kind;                  /* 0 = gradient stage, 1 = Hessian-vector stage */
@@ -514,6 +517,14 @@ int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden,
                                            const promp_policy_stage* stages);
 /* kernels promp_policy_chain launches for these stages with the current options: 1 (dataflow kernel) or n_stages */
 int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages, const promp_policy_stage* stages);
+/*
+ * The work-item plan of the dataflow kernel for these stages under the current chain_q / chain_taper options (reads only
+ * `kind` and `N` of each stage; no device work).  out[0] = SMs the plan is made for, out[1] = items in all, then 15 ints per
+ * stage: ntiles, item_base, n_items, n_regions, reg_m0[4], reg_q[3], reg_item0[3], kind.  Region r is tasks
+ * [reg_m0[r], reg_m0[r+1]) at reg_q[r] tiles per item, its first item at stage-relative id reg_item0[r].  Whether the
+ * dataflow kernel runs is promp_policy_chain_num_launches's answer.
+ */
+int promp_policy_chain_plan_info(int M, int n_stages, const promp_policy_stage* stages, int32_t* out);
 int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
                        const promp_policy_stage* stages, const int32_t* skip_flag, const float* skip_theta,
                        void* workspace, int64_t workspace_bytes, void* stream);

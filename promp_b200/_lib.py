@@ -90,6 +90,7 @@ _SIGNATURES = {
                                         c_float, c_float, c_int, c_float, _P, _P, _P, _P, c_int64, _P]),
     'promp_policy_chain_workspace_bytes': (c_int64, [c_int, c_int, c_int, c_int, c_int, _P]),
     'promp_policy_chain_num_launches': (c_int, [c_int, c_int, c_int, c_int, c_int, _P]),
+    'promp_policy_chain_plan_info': (c_int, [c_int, c_int, _P, _P]),
     'promp_policy_chain': (c_int, [c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, c_int64, _P]),
     'promp_meta_loss_terms': (c_int, [c_int, c_int, _P, c_float, _P, c_int, _P, _P]),
     'promp_phase_log_terms': (c_int, [c_int, c_int, c_double, _P, _P, _P, _P]),

@@ -1060,6 +1060,14 @@ struct ChainPlan {
     int64_t ctrl_bytes, bytes;     // control words (zero on entry, left zero); whole workspace
 };
 static int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
+// Control words at the start of a chain workspace, the same whatever n_stages is (chains of different length share one
+// workspace, and the words must stay zero between calls): work queue and finished-CTA count (4 ints), ready flags and
+// arrival counters of the dataflow kernel ([CHAIN_MAX_STAGES][M] each), then, ending at chain_ctrl_bytes(M), the arrival
+// counters of the one-launch-per-stage path.  Both paths put their partial slots after chain_ctrl_bytes(M), so neither
+// writes scratch over the other's counters.
+static int64_t chain_ctrl_bytes(int M) {
+    return align_up(16 + (int64_t)2 * CHAIN_MAX_STAGES * M * sizeof(int) + counters_bytes(M), 128);
+}
 // Items are (stage, task, q consecutive tiles).  q = the largest of 4, 2, 1 that still gives every stage at least one item
 // per SM; the last stage (nothing left to fill its tail with) uses q, q/2 and 1 on the first half, third quarter and last
 // quarter of its tasks, so the final imbalance over the SMs is one tile.
@@ -1104,8 +1112,7 @@ static ChainPlan plan_chain(int n_stages, const int* kinds, const int* Ns, int M
         base += I.n_items;
     }
     pl.n_items = base;
-    // fixed layout whatever n_stages is: chains of different length share one workspace, and the words must stay zero between them
-    pl.ctrl_bytes = align_up(16 + (int64_t)2 * CHAIN_MAX_STAGES * M * sizeof(int), 128);
+    pl.ctrl_bytes = chain_ctrl_bytes(M);
     pl.bytes = pl.ctrl_bytes + (int64_t)pl.n_items * (P + PSTAT) * sizeof(float);
     return pl;
 }
@@ -1184,9 +1191,11 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
             return has_hvp ? launch_chain_nq<DO, DA, 2, true, Act>(C, st) : launch_chain_nq<DO, DA, 2, false, Act>(C, st);
         }
     }
-    // one launch per stage; their (counters + partial) workspace starts after the chain's control words
-    void* ws1 = (char*)ws + pl.ctrl_bytes;
-    const int64_t ws1_bytes = ws_bytes - pl.ctrl_bytes;
+    // one launch per stage: launch_policy's (counters, partial slots) workspace starts at the last control words, so its
+    // partial slots start at pl.ctrl_bytes
+    const int64_t off1 = pl.ctrl_bytes - counters_bytes(M);
+    void* ws1 = (char*)ws + off1;
+    const int64_t ws1_bytes = ws_bytes - off1;
     for (int s = 0; s < n_stages; ++s) {
         PolicyArgs a = A[s];
         if (s == 0) a.skip_flag = skip_flag, a.skip_theta = skip_theta;
@@ -1522,9 +1531,36 @@ static int chain_stage_args(const promp_policy_stage* stages, int n_stages, int 
     return PROMP_OK;
 }
 
+// the argument check of the chain's size queries; sets last_error
+static bool chain_query_args_ok(const char* who, int M, int n_stages, const promp_policy_stage* stages) {
+    if (stages != nullptr && n_stages >= 1 && n_stages <= CHAIN_MAX_STAGES && M >= 1) return true;
+    set_error("%s: needs M >= 1 and 1..%d stages (got M=%d, %d stages%s)", who, CHAIN_MAX_STAGES, M, n_stages,
+              stages ? "" : ", null stages");
+    return false;
+}
+
+extern "C" int promp_policy_chain_plan_info(int M, int n_stages, const promp_policy_stage* stages, int32_t* out) {
+    if (!chain_query_args_ok("promp_policy_chain_plan_info", M, n_stages, stages)) return PROMP_ERR_INVALID_ARG;
+    PROMP_REQUIRE(out != nullptr, "promp_policy_chain_plan_info: null out");
+    int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
+    for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
+    const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, 0);
+    out[0] = sm_count();
+    out[1] = pl.n_items;
+    for (int s = 0; s < n_stages; ++s) {
+        const ChainStageInfo& I = pl.info[s];
+        int32_t* o = out + 2 + 15 * s;
+        o[0] = I.ntiles, o[1] = I.item_base, o[2] = I.n_items, o[3] = I.n_regions;
+        for (int r = 0; r <= CHAIN_MAX_REGIONS; ++r) o[4 + r] = I.reg_m0[r];
+        for (int r = 0; r < CHAIN_MAX_REGIONS; ++r) o[8 + r] = I.reg_q[r], o[11 + r] = I.reg_item0[r];
+        o[14] = I.kind;
+    }
+    return PROMP_OK;
+}
+
 static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                  const promp_policy_stage* stages) {
-    if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
+    if (!chain_query_args_ok("promp_policy_chain_workspace_bytes", M, n_stages, stages)) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_workspace_bytes")
@@ -1541,7 +1577,7 @@ extern "C" int64_t promp_policy_chain_workspace_bytes_padded(int obs_dim, int ac
 
 static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                           const promp_policy_stage* stages) {
-    if (stages == nullptr || n_stages < 1 || n_stages > CHAIN_MAX_STAGES || M < 1) return -1;
+    if (!chain_query_args_ok("promp_policy_chain_num_launches", M, n_stages, stages)) return -1;
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_num_launches")
@@ -1554,6 +1590,23 @@ extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hid
 extern "C" int promp_policy_chain_num_launches_padded(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                       const promp_policy_stage* stages) {
     return policy_chain_num_launches_impl(true, obs_dim, act_dim, hidden, M, n_stages, stages);
+}
+
+// The control words grow with M: a call with a larger M finds them where a call with a smaller M left partial slots (its
+// arrival counters would start non-zero, no CTA would be a task's last arriver).  So when M changes on a workspace, clear
+// them on the stream first.  An algorithm keeps one M per workspace, so the steady state (and a captured CUDA graph) has no
+// extra node.  Workspaces this record has not seen are cleared once: a fresh one is zero anyway, and one pushed out of the
+// record may have served another M.
+static int chain_clear_on_new_m(void* ws, int M, cudaStream_t st) {
+    static struct { void* ws; int M; } seen[16];
+    static int next = 0;
+    int i = 0;
+    while (i < 16 && seen[i].ws != ws) ++i;
+    if (i < 16 && seen[i].M == M) return PROMP_OK;
+    if (i == 16) i = next, next = (next + 1) % 16;
+    seen[i].ws = ws, seen[i].M = M;
+    PROMP_CUDA(cudaMemsetAsync(ws, 0, chain_ctrl_bytes(M), st));
+    return PROMP_OK;
 }
 
 static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
@@ -1570,6 +1623,13 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
     for (int k = 0; k < n_stages; ++k) A[k].obs_dim = obs_dim, A[k].act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_chain")
+    if (workspace_bytes < chain_ctrl_bytes(M)) {
+        set_error("policy chain workspace too small (%lld < %lld bytes of control words)", (long long)workspace_bytes,
+                  (long long)chain_ctrl_bytes(M));
+        return PROMP_ERR_WORKSPACE;
+    }
+    const int rc_clear = chain_clear_on_new_m(workspace, M, s);
+    if (rc_clear != PROMP_OK) return rc_clear;
     return PROMP_UNIT(chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta, workspace,
                              workspace_bytes, s);
 }

@@ -29,12 +29,17 @@ class MAMLAlgo(object):
     """
     inner_obj_kind = _lib.OBJ_RATIO
     CHAIN_MAX_STAGES = 6          # promp_policy_chain's stage limit
+    MAX_INNER_GRAD_STEPS = 6      # promp_meta_loss_terms / promp_adapt_kl_coeff take at most 7 sampling phases
     STATS_SLOTS = 16              # per-evaluation stats buffers kept per (S, M), see _stats_rows
 
     def __init__(self, policy, inner_lr=0.1, meta_batch_size=20, num_inner_grad_steps=1,
                  trainable_inner_step_size=False):
         assert hasattr(policy, 'sampling_params'), "policy must be a promp_b200 MetaGaussianMLPPolicy"
         assert type(num_inner_grad_steps) and num_inner_grad_steps >= 0
+        if num_inner_grad_steps > self.MAX_INNER_GRAD_STEPS:
+            raise ValueError("num_inner_grad_steps=%d: at most %d inner gradient steps are supported (the device loss-term and "
+                             "KL-coefficient kernels take up to %d sampling phases)"
+                             % (num_inner_grad_steps, self.MAX_INNER_GRAD_STEPS, self.MAX_INNER_GRAD_STEPS + 1))
         assert type(meta_batch_size) == int
         if trainable_inner_step_size:
             raise NotImplementedError("trainable_inner_step_size is not supported (reference: 'it isn't supported "
@@ -140,20 +145,29 @@ class MAMLAlgo(object):
         return st
 
     def _run_chain(self, stages, reuse=None):
-        """promp_policy_chain over a list of PolicyStage (all buffers must stay alive until the launch has run)."""
+        """promp_policy_chain over a list of PolicyStage (all buffers must stay alive until the launch has run).  A list longer
+        than CHAIN_MAX_STAGES (three or more inner steps) runs as consecutive launches of at most CHAIN_MAX_STAGES stages on
+        one stream: stream order is the dependency between them, and each launch leaves the shared workspace's control
+        words zero.  The launch re-use pointers belong to stage 0, so only the first launch gets them."""
         import torch
         p = self.policy
-        arr = (_lib.PolicyStage * len(stages))(*stages)
-        need = getattr(_lib.load(), p.entries['chain_workspace_bytes'])(p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size,
-                                                                        len(stages), ctypes.cast(arr, ctypes.c_void_p))
-        if need < 0:
-            raise _lib.PrompLibraryError(p.entries['chain_workspace_bytes'] + ": " + _lib.last_error())
+        pieces = [(_lib.PolicyStage * len(part))(*part)
+                  for part in (stages[i:i + self.CHAIN_MAX_STAGES] for i in range(0, len(stages), self.CHAIN_MAX_STAGES))]
+        need = 0
+        for arr in pieces:
+            n = getattr(_lib.load(), p.entries['chain_workspace_bytes'])(p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size,
+                                                                         len(arr), ctypes.cast(arr, ctypes.c_void_p))
+            if n < 0:
+                raise _lib.PrompLibraryError(p.entries['chain_workspace_bytes'] + ": " + _lib.last_error())
+            need = max(need, n)
         if self._ws_chain is None or self._ws_chain.numel() * 4 < need:
             self._ws_chain = torch.zeros((need + 3) // 4, dtype=torch.int32, device=p.device)   # control words start at zero
         ws = self._ws_chain
         skip = (_lib.ptr(reuse[0]), _lib.ptr(reuse[1])) if reuse is not None else (None, None)
-        _lib.call(p.entries['chain'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, float(p.min_log_std), len(stages),
-                  ctypes.cast(arr, ctypes.c_void_p), skip[0], skip[1], _lib.ptr(ws), ws.numel() * 4, _lib.stream())
+        for i, arr in enumerate(pieces):
+            _lib.call(p.entries['chain'], p.obs_dim, p.action_dim, p.hidden_arg, self.meta_batch_size, float(p.min_log_std),
+                      len(arr), ctypes.cast(arr, ctypes.c_void_p), skip[0] if i == 0 else None, skip[1] if i == 0 else None,
+                      _lib.ptr(ws), ws.numel() * 4, _lib.stream())
 
     def _hvp(self, phase, params, stride, vec, out, kl_coeff, clip_log_std, stats=None):
         p = self.policy
@@ -283,14 +297,11 @@ class MAMLAlgo(object):
                                               kl_coeff_dev=None if inner_kl_coeffs_dev is None else inner_kl_coeffs_dev[s:s + 1]))
                     chain.append(v)       # the stage list holds raw pointers: keep every buffer alive until the launch is enqueued
                     v = v_out
-            x_separate = explore is not None and len(stages) >= self.CHAIN_MAX_STAGES
-            if explore is not None and not x_separate:
+            if explore is not None:
                 # last stage, waits for no other: in the dataflow kernel it fills the tail of the backward chain
                 stages.append(self._stage(0, phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=x_grad, stats=x_stats,
                                           adv=explore))
             self._run_chain(stages, reuse=self._reuse_bufs if reuse0 else None)
-            if x_separate:
-                explore_launch()
             out = dict(surr=stats_all[S - 1, :, 0], outer_kl=stats_all[S - 1, :, 1], inner_kl=stats_all[:S - 1, :, 1],
                        stats_all=stats_all, grad=None)
             if x_stats is not None:
