@@ -220,6 +220,52 @@ int promp_rollout_early_term_ex(int env_kind, int normalize_actions, int M, int 
                                 int clip_reported_log_std, float min_log_std, float* obs, float* act, float* mean, float* rew,
                                 uint8_t* done, float* log_std_out, void* stream, int task_offset);
 int promp_paths_histogram(int M, int E, int timeline_len, const uint8_t* t_done, int32_t* hist, void* stream);
+
+/*
+ * Users' own environments (promp_b200.envs.CudaMetaEnv): an env struct compiled at run time by NVRTC into the same fused
+ * rollout, env-step and env-observe kernels as the built-in envs (csrc/user_env.cuh, promp_b200/_jit.py).
+ *
+ * promp_env_module_load: loads the cubin `image` (`bytes` long) and resolves its kernels by their lowered names.
+ *   names [PROMP_ENV_MODULE_SLOTS]: slot PROMP_ENV_SLOT_STEP = env_step_kernel, PROMP_ENV_SLOT_OBSERVE = env_observe_kernel,
+ *   PROMP_ENV_SLOT_ROLLOUT + 2*v + keyed = rollout_kernel of `hidden` variant v = (relu + 2*out_tanh)*2 + (width == 64),
+ *   keyed = the sharded (task_offset != 0) instantiation.  NULL or "" = not compiled; launching it returns
+ *   PROMP_ERR_INVALID_ARG.  dims [PROMP_ENV_MODULE_NDIMS] = {obs, act, state, task sizes, info channels, ends early}; obs
+ *   1..19, act 1..8 (the rollout policy's range), info 0..3.  *handle_out: the module, until promp_env_module_unload.
+ *   There is no reference counterpart (the reference steps Python envs, envs/base.py:6-49).
+ * promp_rollout_module: promp_rollout_ex (samplers/meta_sampler.py:59-137 with vectorized_env_executor.py:25-52) for the
+ *   module's env.  info [NINFO, M, E, H] is required when the env writes info channels (channel c as the env wrote it).
+ *   Rejects an env that ends early.
+ * promp_rollout_early_term_module: promp_rollout_early_term_ex (the same reference loop with early `done`) for a module
+ *   whose env ends early; in-kernel resets call the env's reset with Philox draws keyed by (env, step).  The timelines go
+ *   to promp_paths_finalize / promp_paths_finalize_ex unchanged.
+ * promp_env_step_module / promp_env_observe_module: promp_env_step / promp_env_observe (MetaIterativeEnvExecutor.step /
+ *   reset, vectorized_env_executor.py:25-75) for the module's env; info [NINFO, n_env] or NULL.
+ */
+#define PROMP_ENV_MODULE_SLOTS 18
+#define PROMP_ENV_MODULE_NDIMS 6
+#define PROMP_ENV_SLOT_STEP 0
+#define PROMP_ENV_SLOT_OBSERVE 1
+#define PROMP_ENV_SLOT_ROLLOUT 2
+int promp_env_module_load(const void* image, int64_t bytes, const char* const* names, int n_names, const int* dims,
+                          void** handle_out);
+int promp_env_module_unload(void* handle);
+int promp_rollout_module(void* module, int reward_type, float sparse_radius, int normalize_actions, int M, int E, int H,
+                         int hidden, const float* params, int64_t param_stride, const float* task_params, const float* init_state,
+                         const float* noise, uint64_t seed, uint64_t stream_id, const uint64_t* stream_id_dev,
+                         int clip_reported_log_std, float min_log_std, float* obs, float* act, float* mean, float* rew,
+                         uint8_t* done, float* info, float* log_std_out, float* final_state, void* stream, int task_offset);
+int promp_rollout_early_term_module(void* module, int normalize_actions, int M, int E, int timeline_len, int horizon, int hidden,
+                                    const float* params, int64_t param_stride, const float* task_params, const float* init_state,
+                                    const float* noise, uint64_t seed, uint64_t stream_id, const uint64_t* stream_id_dev,
+                                    int clip_reported_log_std, float min_log_std, float* obs, float* act, float* mean,
+                                    float* rew, uint8_t* done, float* log_std_out, void* stream, int task_offset);
+int promp_env_step_module(void* module, int reward_type, float sparse_radius, int normalize_actions, int n_env, int H,
+                          float* state, int32_t* ts, const float* actions, const float* task_params, const float* reset_state,
+                          float* next_obs, float* rew, uint8_t* done, float* info, void* stream);
+int promp_env_observe_module(void* module, int n_env, const float* state, float* obs, void* stream);
+/* CUDART_VERSION the library was built with (e.g. 12090): the JIT prefers an NVRTC of the same version, whose code for
+ * the built-in env types is then the library's own. */
+int promp_cuda_build_version(void);
 int promp_paths_finalize_ex(int M, int E, int timeline_len, int max_paths, int max_samples, int obs_dim, int act_dim,
                             int64_t target_samples, const int32_t* hist_in, const uint8_t* t_done, const float* t_obs,
                             const float* t_act, const float* t_mean, const float* t_rew, int32_t* path_off, int32_t* n_paths,

@@ -12,7 +12,7 @@ CSRC = os.path.join(PKG, 'csrc')
 OBJ = os.path.join(ROOT, 'build', 'obj')
 LIB = os.path.join(PKG, 'libpromp_b200.so')
 SOURCES = ('common.cu', 'rollout.cu', 'process.cu', 'policy.cu', 'policy_relu.cu', 'policy_otanh.cu', 'policy_relu_otanh.cu', 'comm.cu',
-           'trpo.cu', 'paths.cu')
+           'trpo.cu', 'paths.cu', 'env_module.cu')
 NVCC_FLAGS = ['-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 

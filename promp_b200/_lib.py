@@ -16,6 +16,8 @@ ENV_POINT_CORNER, ENV_POINT, ENV_CHEETAH_DIR, ENV_POINT_WALLS, ENV_POINT_MOMENTU
 ENV_WALKER, ENV_SWIMMER = 5, 6
 EARLY_TERM_ENVS = (ENV_POINT, ENV_WALKER)        # env kinds whose paths end on `done` (variable-length paths)
 INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write env_infos channels
+# env modules (promp_env_module_load): kernel slots and dims
+ENV_MODULE_SLOTS, ENV_MODULE_NDIMS, ENV_SLOT_STEP, ENV_SLOT_OBSERVE, ENV_SLOT_ROLLOUT = 18, 6, 0, 1, 2
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE, OBJ_EXPLORE = 0, 1, 2, 3, 4
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE, BASELINE_LINEAR_TIME, BASELINE_GIVEN = 0, 1, 2, 3
@@ -127,6 +129,15 @@ _SIGNATURES = {
                                   c_int, _P, _P, _P, _P, _P]),
     'promp_meta_loss_terms_p2p': (c_int, [c_int, c_int, _P, c_float, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P, _P]),
     'promp_allreduce_p2p': (c_int, [c_int, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P, _P]),
+    'promp_env_module_load': (c_int, [_P, c_int64, _P, c_int, _P, _P]),
+    'promp_env_module_unload': (c_int, [_P]),
+    'promp_rollout_module': (c_int, [_P, c_int, c_float, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, c_uint64,
+                                     c_uint64, _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int]),
+    'promp_rollout_early_term_module': (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P, _P, c_uint64,
+                                                c_uint64, _P, c_int, c_float, _P, _P, _P, _P, _P, _P, _P, c_int]),
+    'promp_env_step_module': (c_int, [_P, c_int, c_float, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    'promp_env_observe_module': (c_int, [_P, c_int, _P, _P, _P]),
+    'promp_cuda_build_version': (c_int, []),
 }
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 

@@ -1,8 +1,12 @@
 // Shared device/host helpers for the promp_b200 kernels (sm_90a).
+// The device parts also compile under NVRTC (__CUDACC_RTC__: user environments, promp_b200/_jit.py); the host-only parts
+// (error plumbing, argument decoding) are left out there.
 #pragma once
+#ifndef __CUDACC_RTC__
 #include <cuda_runtime.h>
-#include <stdint.h>
 #include <stdio.h>
+#endif
+#include <stdint.h>
 #include "../../include/promp_b200.h"
 
 namespace promp {
@@ -10,6 +14,7 @@ namespace promp {
 // SM count of the target GPU (H100 SXM) for the launch-size heuristics that are fixed at compile time
 constexpr int PROMP_NUM_SMS = 132;
 
+#ifndef __CUDACC_RTC__
 // ---------------------------------------------------------------- error plumbing (host)
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
@@ -33,6 +38,7 @@ int check_cuda(cudaError_t e, const char* what);
         int _st = promp::check_cuda(cudaGetLastError(), name);     \
         if (_st != PROMP_OK) return _st;                           \
     } while (0)
+#endif
 
 // ---------------------------------------------------------------- parameter layout
 // Flat parameter vector in the reference's creation order
@@ -151,6 +157,7 @@ __device__ __forceinline__ void out_hvp_back(const float (&mu)[DA], const float 
     }
 }
 
+#ifndef __CUDACC_RTC__
 // The `hidden` argument of the policy and rollout entry points: the width (32 or 64) in the low byte, PROMP_ACT_RELU and
 // PROMP_OUT_TANH above it.  A plain width selects tanh hidden layers and the identity output.
 inline int decode_hidden(const char* who, int hidden, int& width, bool& relu, bool& out_tanh) {
@@ -166,6 +173,15 @@ inline int decode_hidden(const char* who, int hidden, int& width, bool& relu, bo
                   who, width);
     return PROMP_OK;
 }
+
+// The Philox key of an env is its global index (task_offset + m) * E + e, a 32-bit word (rollout entry points)
+inline int check_task_offset(const char* fn, int task_offset, int M, int E) {
+    PROMP_REQUIRE(task_offset >= 0, "%s: task_offset must be >= 0 (got %d)", fn, task_offset);
+    PROMP_REQUIRE(((int64_t)task_offset + M) * E <= ((int64_t)1 << 32),
+                  "%s: (task_offset + M) * E = (%d + %d) * %d exceeds the 32-bit Philox env key", fn, task_offset, M, E);
+    return PROMP_OK;
+}
+#endif
 
 // ---------------------------------------------------------------- warp helpers
 __device__ __forceinline__ float warp_sum(float v) {

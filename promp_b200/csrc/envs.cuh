@@ -16,7 +16,7 @@
 //   TD (floats per task), NINFO (env_infos channels), NACC (rollout layer-1 accumulators: 2 where the env's registers
 //   leave no room for 4), ENDS_EARLY (the env reports `done` before the horizon);
 //   warp-resident state for rollout_kernel, one warp per env:
-//     load(init_state row, lane), reset(rng, step, tag, lane) (Philox draw), observe(shared obs line, lane),
+//     load(init_state row, lane), reset(rng, step, tag, lane, task) (Philox draw), observe(shared obs line, lane),
 //     step(a, task, cfg, lane, info, info_stride, done) -> reward, store(final_state row, lane);
 //   one thread per env for env_step_kernel / env_observe_kernel:
 //     step_serial(st[SD], a, task, cfg, info, info_stride, done) -> reward, observe_serial(st, obs).
@@ -99,7 +99,7 @@ struct Replicated {
 // counter `step`.
 template <class Env, int SD>
 struct PointState : Replicated<Env, SD> {
-    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int) {
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int, const float*) {
         uint32_t r[4];
         rng.gen(step, tag, r);
         const float lim = Env::RESET_LIM;
@@ -413,7 +413,7 @@ struct Cheetah : Planar9<false> {
 
     // reset_model (half_cheetah_rand_direc.py:49-53): qpos = U(-.1,.1)^9, qvel = .1*N(0,1)^9; lane i < 9 draws coordinate
     // i from counter (step << 4) + i
-    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane) {
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane, const float*) {
         float pos = 0.f, vel = 0.f;
         if (lane < 9) {
             uint32_t r[4];
@@ -576,7 +576,7 @@ struct Walker : Planar9<true> {
 
     // reset_model (walker2d_rand_*.py:47-52): qpos = init_qpos + U(-.005,.005)^9 (init_qpos z = 1.25, all else 0),
     // qvel = U(-.005,.005)^9; lane i < 9 draws coordinate i from counter (step << 4) + i
-    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane) {
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int lane, const float*) {
         float pos = 0.f, vel = 0.f;
         if (lane < 9) {
             uint32_t r[4];
@@ -652,7 +652,7 @@ struct Swimmer : Replicated<Swimmer, 10> {
     static constexpr bool ENDS_EARLY = false;
 
     // reset_model (swimmer_rand_vel.py:41-46): qpos = U(-.1,.1)^5, qvel = U(-.1,.1)^5 from counters (step << 4) + 0..2
-    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int) {
+    __device__ __forceinline__ void reset(const EnvRng& rng, uint32_t step, uint32_t tag, int, const float*) {
 #pragma unroll
         for (int blk = 0; blk < 3; ++blk) {
             uint32_t r[4];

@@ -8,3 +8,4 @@ from promp_b200.envs.point_env_2d_walls import MetaPointEnvWalls  # noqa: F401
 from promp_b200.envs.point_env_2d_momentum import MetaPointEnvMomentum  # noqa: F401
 from promp_b200.envs.walker2d_rand_vel import Walker2DRandVelEnv, Walker2DRandDirecEnv  # noqa: F401
 from promp_b200.envs.swimmer_rand_vel import SwimmerRandVelEnv  # noqa: F401
+from promp_b200.envs.cuda_env import CudaMetaEnv, CudaEnvProgram  # noqa: F401

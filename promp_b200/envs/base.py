@@ -51,10 +51,14 @@ class MetaEnv(object):
 
     # ---- device description -------------------------------------------------------------
     def device_spec(self):
+        """env_kind (a built-in) or module (a user env, envs/cuda_env.py); ends_early: paths end on `done`; ninfo: env-info
+        channels the kernels write."""
+        info = len(getattr(self, 'info_keys', ('reward_run', 'reward_ctrl'))) if self.env_kind in _lib.INFO_ENVS else 0
         return dict(env_kind=self.env_kind, reward_type=self.reward_type, radius=float(self.sparse_reward_radius),
                     obs_dim=self.obs_dim, act_dim=self.act_dim,
                     state_dim=_lib.load().promp_env_state_dim(self.env_kind),
-                    task_dim=_lib.load().promp_env_task_dim(self.env_kind))
+                    task_dim=_lib.load().promp_env_task_dim(self.env_kind),
+                    ends_early=self.env_kind in _lib.EARLY_TERM_ENVS, ninfo=info)
 
     def task_vector(self, task):
         """float32 vector handed to the kernels for one task."""

@@ -17,7 +17,8 @@ class NormalizedEnv(object):
         if float(normalization_scale) != 10.0:
             raise NotImplementedError("promp_b200: the device env kernels implement normalization_scale=10 only")
         if not hasattr(env, 'device_spec'):
-            raise TypeError("promp_b200.normalize needs a device env (promp_b200.envs.*); got %r" % (env,))
+            raise TypeError("promp_b200.normalize needs a device env (promp_b200.envs.*, or your own dynamics as a "
+                            "promp_b200.envs.CudaMetaEnv); got %r" % (env,))
         self._wrapped_env = env
         self._normalization_scale = normalization_scale
         self._scale_reward = 1

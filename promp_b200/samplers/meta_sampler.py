@@ -66,6 +66,8 @@ class MetaSampler(object):
             self.vec_env = MetaDeviceEnvExecutor(env, self.meta_batch_size, self.envs_per_task, self.max_path_length)
             self.spec = self.vec_env.spec
             self.device = self.vec_env.device
+            if self.spec.get('module') is not None and hasattr(policy, 'hidden_arg'):
+                self.spec['module'].handle(policy.hidden_arg)     # a user env: its rollout kernels, loaded before any capture
         else:
             # duck-typed host env (the reference's test fakes, tests/test_samplers.py:13-67): stepped where Python runs,
             # one env.step per env per step like the reference's iterative executor - slow by construction
@@ -86,14 +88,14 @@ class MetaSampler(object):
 
     def _fused_ok(self):
         return (self.spec is not None and hasattr(self.policy, 'sampling_params')
-                and self.spec['env_kind'] not in _lib.EARLY_TERM_ENVS and self.envs_per_task == self.batch_size)
+                and not self.spec['ends_early'] and self.envs_per_task == self.batch_size)
 
     def _fused_early_ok(self):
         """Early-terminating envs (MetaPointEnv, the Walker2d surrogates) through the fused kernel + device-side path table.
         Opt-in via reset_mode='device': in-kernel resets cannot follow the host numpy stream (their number is data-dependent),
         so reset_mode='numpy' keeps the reference's step loop with host draws."""
         return (self.spec is not None and hasattr(self.policy, 'sampling_params')
-                and self.spec['env_kind'] in _lib.EARLY_TERM_ENVS
+                and self.spec['ends_early']
                 and self.reset_mode == 'device' and self.envs_per_task == self.batch_size and self.envs_per_task <= 1024)
 
     def obtain_samples(self, log=False, log_prefix=''):
@@ -120,7 +122,7 @@ class MetaSampler(object):
         s = self.spec
         M, E, H = self.meta_batch_size, self.envs_per_task, self.max_path_length
         params, stride, clip = self.policy.sampling_params()
-        if s['env_kind'] in _lib.INFO_ENVS and phase.info is None:
+        if s['ninfo'] and phase.info is None:
             keys = tuple(getattr(getattr(self.env, '_wrapped_env', self.env), 'info_keys', ('reward_run', 'reward_ctrl')))
             phase.info = torch.empty(len(keys), M, E * H, dtype=torch.float32, device=self.device)
             phase.info_keys = keys
@@ -131,7 +133,9 @@ class MetaSampler(object):
                 float(self.policy.min_log_std),
                 _lib.ptr(phase.obs), _lib.ptr(phase.act), _lib.ptr(phase.mean), _lib.ptr(phase.rew),
                 _lib.ptr(phase.done), _lib.ptr(phase.info), _lib.ptr(phase.log_std), None, _lib.stream())
-        if self._shard_world > 1:
+        if s.get('module') is not None:
+            _lib.call('promp_rollout_module', s['module'].handle(self.policy.hidden_arg), *args[1:], self._task_offset)
+        elif self._shard_world > 1:
             _lib.call('promp_rollout_ex', *args, self._task_offset)
         else:
             _lib.call('promp_rollout', *args)
@@ -279,7 +283,9 @@ class MetaSampler(object):
                 self._phase_counter, _lib.ptr(self._phase_counter_dev), clip, float(self.policy.min_log_std), _lib.ptr(tl['obs']),
                 _lib.ptr(tl['act']), _lib.ptr(tl['mean']), _lib.ptr(tl['rew']), _lib.ptr(tl['done']), _lib.ptr(phase.log_std),
                 _lib.stream())
-        if self._shard_world > 1:
+        if s.get('module') is not None:
+            _lib.call('promp_rollout_early_term_module', s['module'].handle(self.policy.hidden_arg), *args[1:], self._task_offset)
+        elif self._shard_world > 1:
             _lib.call('promp_rollout_early_term_ex', *args, self._task_offset)
         else:
             _lib.call('promp_rollout_early_term', *args)

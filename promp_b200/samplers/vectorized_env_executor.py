@@ -34,7 +34,8 @@ class MetaDeviceEnvExecutor(object):
         self._rew = torch.zeros(self.n_envs, **f32)
         self._done = torch.zeros(self.n_envs, dtype=torch.uint8, device=self.device)
         inner_env = getattr(env, '_wrapped_env', env)
-        self.info_keys = tuple(getattr(inner_env, 'info_keys', ())) if self.spec['env_kind'] in _lib.INFO_ENVS else ()
+        self.info_keys = tuple(getattr(inner_env, 'info_keys', ())) if self.spec['ninfo'] else ()
+        self._module = self.spec.get('module')      # a user env (envs/cuda_env.py): its env-step / env-observe kernels
         self._info = torch.zeros(max(len(self.info_keys), 2), self.n_envs, **f32)
         self._dummy_reset = torch.zeros(self.n_envs, sd, **f32)
 
@@ -55,8 +56,12 @@ class MetaDeviceEnvExecutor(object):
             self.env.set_task(tasks[-1])
 
     def _observe(self):
-        _lib.call('promp_env_observe', self.spec['env_kind'], self.n_envs, _lib.ptr(self.state), _lib.ptr(self._obs),
-                  _lib.stream())
+        if self._module is not None:
+            _lib.call('promp_env_observe_module', self._module.handle(), self.n_envs, _lib.ptr(self.state), _lib.ptr(self._obs),
+                      _lib.stream())
+        else:
+            _lib.call('promp_env_observe', self.spec['env_kind'], self.n_envs, _lib.ptr(self.state), _lib.ptr(self._obs),
+                      _lib.stream())
 
     def reset(self):
         """vectorized_env_executor.py:66-75: reset states drawn on the host numpy RNG in env order."""
@@ -77,8 +82,9 @@ class MetaDeviceEnvExecutor(object):
             self._per_env_tasks_stale = False
         act = torch.from_numpy(np.asarray(actions, dtype=np.float32).reshape(self.n_envs, -1)).to(self.device)
         s = self.spec
-        _lib.call('promp_env_step', s['env_kind'], s['reward_type'], s['radius'], int(s.get('normalized', False)), self.n_envs,
-                  self.max_path_length,
+        _lib.call('promp_env_step_module' if self._module is not None else 'promp_env_step',
+                  self._module.handle() if self._module is not None else s['env_kind'], s['reward_type'], s['radius'],
+                  int(s.get('normalized', False)), self.n_envs, self.max_path_length,
                   _lib.ptr(self.state), _lib.ptr(self.ts), _lib.ptr(act), _lib.ptr(self.task_params),
                   _lib.ptr(self._dummy_reset), _lib.ptr(self._obs), _lib.ptr(self._rew), _lib.ptr(self._done),
                   _lib.ptr(self._info), _lib.stream())
