@@ -388,6 +388,28 @@ int promp_meta_update(int M, int P, const float* task_grads, float scale, float*
                       int32_t* step, float lr, float beta1, float beta2, float eps, int world, int rank, int capacity_floats,
                       void* const* peers_dev, uint32_t* epoch_dev, uint32_t* error_flag_dev, uint32_t* ticket_dev, void* stream);
 
+/*
+ * Meta-SGD (trainable per-parameter inner step sizes alpha [P], shared by all tasks and inner steps): the fused outer update
+ * over the concatenated gradient [theta; alpha] (2P values).  Per element,
+ *   grad_theta = scale * sum_m task_grads[m]                                (as promp_meta_update)
+ *   grad_alpha = -scale * sum_m sum_s lam[s][m] * g[s][m]
+ * where, for inner step s, lam[s] [M, P] is the direction that enters the Hessian-vector stage of step s and g[s] [M, P] is
+ * the inner gradient of step s (theta_{s+1} = theta_s - alpha * g[s]); lam / g are HOST arrays of n_pairs (0..6) device
+ * pointers.  Then ONE exchange of the 2P values over the peer buffers (world > 1, capacity >= 2P) and TF1 Adam on theta
+ * (slots m, v) and alpha (slots m_alpha, v_alpha) with one step counter, incremented once.  grad_out [2P] or NULL.
+ * grad_in [2P] non-NULL: the summed gradient is given (world must be 1; task_grads / lam / g are not read) and only Adam runs:
+ * the NCCL path, after promp_reduce_tasks_sgd and an all-reduce.
+ * promp_reduce_tasks_sgd: out [2P] = the local [grad_theta; grad_alpha] above; task_grads NULL: only out[P, 2P) (alpha).
+ * n_pairs = 0 (no inner step) gives a zero alpha gradient.
+ */
+int promp_reduce_tasks_sgd(int M, int P, const float* task_grads, int n_pairs, const float* const* lam, const float* const* g,
+                           float scale, float* out, void* stream);
+int promp_meta_update_sgd(int M, int P, const float* task_grads, int n_pairs, const float* const* lam, const float* const* g,
+                          const float* grad_in, float scale, float* grad_out, float* theta, float* alpha, float* m, float* v,
+                          float* m_alpha, float* v_alpha, int32_t* step, float lr, float beta1, float beta2, float eps, int world,
+                          int rank, int capacity_floats, void* const* peers_dev, uint32_t* epoch_dev, uint32_t* error_flag_dev,
+                          uint32_t* ticket_dev, void* stream);
+
 /* promp_meta_loss_terms with the sum over ranks fused in (world >= 2): local means -> peer exchange -> rank-ordered sum ->
  * KL penalty.  One launch instead of terms + all-reduce + elementwise glue. */
 int promp_meta_loss_terms_p2p(int S, int M, const float* stats_all, float inv_m_global, const float* coeff, int n_out, float* out,
@@ -558,6 +580,10 @@ typedef struct {
     float* stats;                  /* [M,4] or NULL */
     const float* kl_coeff_dev;     /* NULL, or a device float: the stage uses kl_coeff * (*kl_coeff_dev) (device-resident
                                       adaptive coefficient, see promp_adapt_kl_coeff) */
+    const float* step_size;        /* NULL, or per-parameter inner step sizes alpha [P] (device; Meta-SGD,
+                                      trainable_inner_step_size): a gradient stage writes out_params = params - alpha * grad
+                                      (sgd_lr unused); an HVP stage computes vec - inner_lr * H (alpha * vec) + kl_coeff * grad KL
+                                      (pass inner_lr = 1) */
 } promp_policy_stage;
 int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                            const promp_policy_stage* stages);

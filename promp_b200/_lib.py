@@ -33,7 +33,8 @@ class PolicyStage(ctypes.Structure):
                 ('obs', _P), ('act', _P), ('adv', _P), ('old_mean', _P), ('old_log_std', _P),
                 ('ls_per_sample', c_int32), ('obj_kind', c_int32), ('obj_scale', c_float), ('clip_eps', c_float),
                 ('kl_coeff', c_float), ('clip_log_std', c_int32), ('grad', _P), ('out_params', _P), ('sgd_lr', c_float),
-                ('inner_lr', c_float), ('vec', _P), ('out', _P), ('stats', _P), ('kl_coeff_dev', _P)]
+                ('inner_lr', c_float), ('vec', _P), ('out', _P), ('stats', _P), ('kl_coeff_dev', _P),
+                ('step_size', _P)]
 
 
 _SIGNATURES = {
@@ -127,6 +128,9 @@ _SIGNATURES = {
     'promp_ipc_close_handle': (c_int, [_P]),
     'promp_meta_update': (c_int, [c_int, c_int, _P, c_float, _P, _P, _P, _P, _P, c_float, c_float, c_float, c_float, c_int, c_int,
                                   c_int, _P, _P, _P, _P, _P]),
+    'promp_reduce_tasks_sgd': (c_int, [c_int, c_int, _P, c_int, _P, _P, c_float, _P, _P]),
+    'promp_meta_update_sgd': (c_int, [c_int, c_int, _P, c_int, _P, _P, _P, c_float, _P, _P, _P, _P, _P, _P, _P, _P, c_float,
+                                      c_float, c_float, c_float, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     'promp_meta_loss_terms_p2p': (c_int, [c_int, c_int, _P, c_float, _P, c_int, _P, c_int, c_int, c_int, _P, _P, _P, _P]),
     'promp_allreduce_p2p': (c_int, [c_int, c_int, c_int, c_int, _P, _P, c_float, _P, _P, _P, _P, _P]),
     'promp_env_module_load': (c_int, [_P, c_int64, _P, c_int, _P, _P]),
@@ -184,6 +188,11 @@ def ptr(t):
     if not t.is_contiguous():
         raise PrompLibraryError("promp_b200 kernels need contiguous tensors")
     return t.data_ptr()
+
+
+def ptr_array(tensors):
+    """Host array of device pointers (the lam / g arguments of promp_meta_update_sgd / promp_reduce_tasks_sgd)."""
+    return (c_void_p * max(len(tensors), 1))(*[ptr(t) for t in tensors])
 
 
 def stream():

@@ -114,31 +114,34 @@ struct MetaUpdateArgs {
     unsigned int* ticket;
 };
 
+// task sum of column `col` of an [M, P] array in task order (bit-identical to promp_reduce_tasks), 16 independent L2 loads in
+// flight per round trip
+__device__ __forceinline__ float task_sum(const float* col, int M, int P) {
+    float g = 0.f;
+    int m = 0;
+    for (; m + 16 <= M; m += 16) {
+        float x[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) x[u] = __ldcg(col + (int64_t)(m + u) * P);
+#pragma unroll
+        for (int u = 0; u < 16; ++u) g += x[u];
+    }
+    {
+        float x[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) x[u] = (m + u < M) ? __ldcg(col + (int64_t)(m + u) * P) : 0.f;
+#pragma unroll
+        for (int u = 0; u < 16; ++u)
+            if (m + u < M) g += x[u];
+    }
+    return g;
+}
+
 __global__ void __launch_bounds__(256) meta_update_kernel(MetaUpdateArgs A) {
     const int tid = threadIdx.x, b = blockIdx.x, p = b * 256 + tid;
     const int t = *A.step + 1;
     float g = 0.f;
-    if (p < A.P) {
-        // task sum in task order (bit-identical to promp_reduce_tasks), 16 independent L2 loads in flight per round trip
-        const float* col = A.v + p;
-        int m = 0;
-        for (; m + 16 <= A.M; m += 16) {
-            float x[16];
-#pragma unroll
-            for (int u = 0; u < 16; ++u) x[u] = __ldcg(col + (int64_t)(m + u) * A.P);
-#pragma unroll
-            for (int u = 0; u < 16; ++u) g += x[u];
-        }
-        {
-            float x[16];
-#pragma unroll
-            for (int u = 0; u < 16; ++u) x[u] = (m + u < A.M) ? __ldcg(col + (int64_t)(m + u) * A.P) : 0.f;
-#pragma unroll
-            for (int u = 0; u < 16; ++u)
-                if (m + u < A.M) g += x[u];
-        }
-        g *= A.scale;
-    }
+    if (p < A.P) g = task_sum(A.v + p, A.M, A.P) * A.scale;
     uint32_t epoch = 0;
     if (A.world > 1) {
         epoch = *A.epoch_ptr + 1;
@@ -166,6 +169,109 @@ __global__ void __launch_bounds__(256) meta_update_kernel(MetaUpdateArgs A) {
         __threadfence();
         const unsigned int old = atomicAdd(A.ticket, 1u);
         if (old == gridDim.x - 1) {          // every CTA has read step / epoch before taking its ticket
+            *A.step = t;
+            if (A.world > 1) *A.epoch_ptr = epoch;
+            *A.ticket = 0u;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Meta-SGD (trainable per-parameter inner step sizes alpha): the same fused outer update over the concatenated gradient
+// [theta; alpha] (2P values), one Adam step counter for both.  Element e < P is theta's task mean, as in meta_update_kernel;
+// element P + i is alpha's gradient
+//   dJ/dalpha_i = -scale * sum_m sum_s lam_s[m, i] * g_s[m, i]
+// (lam_s = the direction entering HVP stage s, g_s = the inner gradient of stage s: theta_{s+1} = theta_s - alpha * g_s).
+// With grad_in set, the summed [2P] gradient is given (the NCCL path: promp_reduce_tasks_sgd + all-reduce) and only Adam runs.
+constexpr int SGD_MAX_PAIRS = 6;
+struct MetaUpdateSgdArgs {
+    int M, P, n_pairs;
+    const float* v;                        // [M, P] per-task theta gradients (local tasks)
+    const float* lam[SGD_MAX_PAIRS];       // [M, P] each
+    const float* gs[SGD_MAX_PAIRS];        // [M, P] each
+    const float* grad_in;                  // [2P] or NULL
+    float scale;                           // 1 / (M * world)
+    float* grad_out;                       // [2P] or NULL
+    float* prm[2]; float* mm[2]; float* vv[2];     // theta / alpha and their Adam slots
+    int32_t* step;
+    float lr, b1, b2, eps;
+    int world, rank, cap;
+    float* const* peers; uint32_t* epoch_ptr; uint32_t* error_flag;
+    unsigned int* ticket;
+};
+
+// element e of the local [theta; alpha] gradient (scaled, not yet summed over ranks)
+__device__ __forceinline__ float sgd_local_grad(const MetaUpdateSgdArgs& A, int e) {
+    if (e < A.P) return task_sum(A.v + e, A.M, A.P) * A.scale;
+    // per task the sum over inner steps, then the tasks in task order; 4 tasks' loads in flight per round trip
+    constexpr int U = 4;
+    const int i = e - A.P;
+    float g = 0.f;
+#pragma unroll 1
+    for (int m0 = 0; m0 < A.M; m0 += U) {
+        float t[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) t[u] = 0.f;
+#pragma unroll
+        for (int s = 0; s < SGD_MAX_PAIRS; ++s) {
+            if (s >= A.n_pairs) break;
+            float l[U], x[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+                const int64_t o = (int64_t)(m0 + u) * A.P + i;
+                l[u] = m0 + u < A.M ? __ldcg(A.lam[s] + o) : 0.f;
+                x[u] = m0 + u < A.M ? __ldcg(A.gs[s] + o) : 0.f;
+            }
+#pragma unroll
+            for (int u = 0; u < U; ++u) t[u] = fmaf(l[u], x[u], t[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < U; ++u)
+            if (m0 + u < A.M) g += t[u];
+    }
+    return -g * A.scale;
+}
+
+__global__ void __launch_bounds__(256) reduce_tasks_sgd_kernel(MetaUpdateSgdArgs A, int e0) {
+    const int e = e0 + blockIdx.x * 256 + threadIdx.x;
+    if (e < 2 * A.P) A.grad_out[e] = sgd_local_grad(A, e);
+}
+
+__global__ void __launch_bounds__(256) meta_update_sgd_kernel(MetaUpdateSgdArgs A) {
+    const int tid = threadIdx.x, e = blockIdx.x * 256 + tid;
+    const int t = *A.step + 1;
+    const int n = 2 * A.P;
+    float g = 0.f;
+    if (e < n) g = A.grad_in ? A.grad_in[e] : sgd_local_grad(A, e);
+    uint32_t epoch = 0;
+    if (A.world > 1) {          // one exchange of the whole [theta; alpha] vector per Adam epoch
+        epoch = *A.epoch_ptr + 1;
+        const int slot = epoch & 1;
+        if (e < n) {
+            ll_send(A.peers, A.world, A.rank, A.cap, slot, e, g, epoch);
+            float s;
+            g = (*reinterpret_cast<volatile uint32_t*>(A.error_flag) == 0 &&
+                 ll_recv_sum(A.peers, A.world, A.rank, A.cap, slot, e, epoch, A.error_flag, &s)) ? s : __int_as_float(0x7fc00000);
+        }
+    }
+    if (e < n) {
+        if (A.grad_out) A.grad_out[e] = g;
+        const int h = e >= A.P, p = e - h * A.P;
+        float* const th = A.prm[h];
+        float* const mm = A.mm[h];
+        float* const vv = A.vv[h];
+        const float lr_t = A.lr * sqrtf(1.f - powf(A.b2, (float)t)) / (1.f - powf(A.b1, (float)t));
+        const float mn = A.b1 * mm[p] + (1.f - A.b1) * g;
+        const float vn = A.b2 * vv[p] + (1.f - A.b2) * g * g;
+        mm[p] = mn;
+        vv[p] = vn;
+        th[p] = th[p] - lr_t * mn / (sqrtf(vn) + A.eps);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        __threadfence();
+        const unsigned int old = atomicAdd(A.ticket, 1u);
+        if (old == gridDim.x - 1) {
             *A.step = t;
             if (A.world > 1) *A.epoch_ptr = epoch;
             *A.ticket = 0u;
@@ -278,6 +384,65 @@ extern "C" int promp_meta_update(int M, int P, const float* task_grads, float sc
                      reinterpret_cast<float* const*>(peers_dev), epoch_dev, error_flag_dev, ticket_dev};
     meta_update_kernel<<<(P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(A);
     PROMP_LAUNCH_CHECK("meta_update_kernel");
+    return PROMP_OK;
+}
+
+static int sgd_pairs(MetaUpdateSgdArgs& A, const char* who, int M, int P, const float* task_grads, int n_pairs,
+                     const float* const* lam, const float* const* g) {
+    PROMP_REQUIRE(M > 0 && P > 0 && n_pairs >= 0 && n_pairs <= SGD_MAX_PAIRS && (n_pairs == 0 || (lam && g)),
+                  "%s: bad arguments (0 <= n_pairs <= %d)", who, SGD_MAX_PAIRS);
+    A.M = M; A.P = P; A.n_pairs = n_pairs; A.v = task_grads;
+    for (int s = 0; s < n_pairs; ++s) {
+        PROMP_REQUIRE(lam[s] && g[s], "%s: pair %d has a null pointer", who, s);
+        A.lam[s] = lam[s];
+        A.gs[s] = g[s];
+    }
+    return PROMP_OK;
+}
+
+// task_grads NULL: only the alpha half out[P, 2P) is written (the theta half comes from promp_reduce_tasks / _tasks2)
+extern "C" int promp_reduce_tasks_sgd(int M, int P, const float* task_grads, int n_pairs, const float* const* lam,
+                                      const float* const* g, float scale, float* out, void* stream) {
+    MetaUpdateSgdArgs A{};
+    const int st = sgd_pairs(A, "promp_reduce_tasks_sgd", M, P, task_grads, n_pairs, lam, g);
+    if (st != PROMP_OK) return st;
+    PROMP_REQUIRE(out, "promp_reduce_tasks_sgd: null output");
+    A.scale = scale; A.grad_out = out;
+    const int e0 = task_grads ? 0 : P;
+    reduce_tasks_sgd_kernel<<<(2 * P - e0 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(A, e0);
+    PROMP_LAUNCH_CHECK("reduce_tasks_sgd_kernel");
+    return PROMP_OK;
+}
+
+extern "C" int promp_meta_update_sgd(int M, int P, const float* task_grads, int n_pairs, const float* const* lam,
+                                     const float* const* g, const float* grad_in, float scale, float* grad_out, float* theta,
+                                     float* alpha, float* m, float* v, float* m_alpha, float* v_alpha, int32_t* step, float lr,
+                                     float beta1, float beta2, float eps, int world, int rank, int capacity_floats,
+                                     void* const* peers_dev, uint32_t* epoch_dev, uint32_t* error_flag_dev, uint32_t* ticket_dev,
+                                     void* stream) {
+    MetaUpdateSgdArgs A{};
+    if (grad_in) {
+        PROMP_REQUIRE(P > 0 && world == 1, "promp_meta_update_sgd: a given gradient needs P > 0 and world == 1");
+        A.P = P; A.grad_in = grad_in;
+    } else {
+        const int st = sgd_pairs(A, "promp_meta_update_sgd", M, P, task_grads, n_pairs, lam, g);
+        if (st != PROMP_OK) return st;
+    }
+    PROMP_REQUIRE(theta && alpha && m && v && m_alpha && v_alpha && step && ticket_dev, "promp_meta_update_sgd: null pointer argument");
+    PROMP_REQUIRE(2 * P <= 256 * COMM_MAX_SLICES, "promp_meta_update_sgd: 2P=%d exceeds %d values", 2 * P, 256 * COMM_MAX_SLICES);
+    PROMP_REQUIRE(world >= 1 && world <= 64 && rank >= 0 && rank < world, "promp_meta_update_sgd: bad world/rank");
+    if (world > 1) {
+        PROMP_REQUIRE(peers_dev && epoch_dev && error_flag_dev && 2 * P <= capacity_floats,
+                      "promp_meta_update_sgd: multi-rank call needs the peer table, epoch / error words and capacity >= 2P");
+    }
+    A.scale = scale; A.grad_out = grad_out;
+    A.prm[0] = theta; A.prm[1] = alpha; A.mm[0] = m; A.mm[1] = m_alpha; A.vv[0] = v; A.vv[1] = v_alpha;
+    A.step = step; A.lr = lr; A.b1 = beta1; A.b2 = beta2; A.eps = eps;
+    A.world = world; A.rank = rank; A.cap = capacity_floats;
+    A.peers = reinterpret_cast<float* const*>(peers_dev); A.epoch_ptr = epoch_dev; A.error_flag = error_flag_dev;
+    A.ticket = ticket_dev;
+    meta_update_sgd_kernel<<<(2 * P + 255) / 256, 256, 0, (cudaStream_t)stream>>>(A);
+    PROMP_LAUNCH_CHECK("meta_update_sgd_kernel");
     return PROMP_OK;
 }
 

@@ -34,8 +34,7 @@ struct PolicyArgs {
     int clip_log_std;
     float min_log_std;
     int obs_dim;         // logical observation / action sizes; read only by the padded instantiations (IsBucket below).  Both
-                         // sit in what was alignment padding: the struct's size and field offsets, and so the parameter
-                         // layout of every kernel taking PolicyArgs or ChainArgs, are unchanged.
+                         // sit in what was alignment padding.
     // grad kernel
     float* grad;
     float* out_params;
@@ -65,8 +64,12 @@ struct PolicyArgs {
     // optional device-resident multiplier of kl_coeff (ProMP's adaptive inner-KL coefficient lives on the device so that an
     // iteration has no host decision: promp_adapt_kl_coeff updates it between launches)
     const float* kl_coeff_ptr;
+    // optional per-parameter inner step sizes alpha [P] (Meta-SGD, trainable_inner_step_size): the gradient kernels' SGD step is
+    // params - alpha * grad in place of params - sgd_lr * grad, and the HVP kernels stage the direction as alpha * vec (the
+    // caller passes inner_lr = 1).  nullptr = the scalar forms.
+    const float* step_size;
 };
-static_assert(sizeof(PolicyArgs) == 224 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120 &&
+static_assert(sizeof(PolicyArgs) == 232 && offsetof(PolicyArgs, grad) == 96 && offsetof(PolicyArgs, vec) == 120 &&
                   offsetof(PolicyArgs, stats) == 144,
               "PolicyArgs layout");
 
@@ -473,7 +476,7 @@ __device__ __forceinline__ void hvp_signal(const HeadIn<DA>& hin, const HeadOut<
 // stores float4 column p of the task's summed slots.
 template <int P, class Sched>
 struct GradEpilogue {      // grad = sum ; out_params = params - sgd_lr * grad   (meta_algos/base.py:209)
-    const PolicyArgs& A;
+    const PolicyArgs& A;   // or params - alpha * grad with per-parameter step sizes (A.step_size)
     const float* th;
     int m;
     __device__ __forceinline__ float4 pre(int p) const {
@@ -481,9 +484,15 @@ struct GradEpilogue {      // grad = sum ; out_params = params - sgd_lr * grad  
     }
     __device__ __forceinline__ void out(int p, float4 t, float4 s) const {
         *reinterpret_cast<float4*>(A.grad + (int64_t)m * P + p) = s;
-        if (A.out_params)
-            *reinterpret_cast<float4*>(A.out_params + (int64_t)m * P + p) =
-                make_float4(t.x - A.sgd_lr * s.x, t.y - A.sgd_lr * s.y, t.z - A.sgd_lr * s.z, t.w - A.sgd_lr * s.w);
+        if (A.out_params) {
+            float4* o = reinterpret_cast<float4*>(A.out_params + (int64_t)m * P + p);
+            if (A.step_size) {
+                const float4 a = __ldg(reinterpret_cast<const float4*>(A.step_size + p));
+                *o = make_float4(t.x - a.x * s.x, t.y - a.y * s.y, t.z - a.z * s.z, t.w - a.w * s.w);
+            } else {
+                *o = make_float4(t.x - A.sgd_lr * s.x, t.y - A.sgd_lr * s.y, t.z - A.sgd_lr * s.z, t.w - A.sgd_lr * s.w);
+            }
+        }
     }
 };
 template <int P>

@@ -433,7 +433,8 @@ __device__ __forceinline__ void policy_hvp_body(const PolicyArgs& A) {
         __syncthreads();
         for (int i = tid; i < L::P; i += PT_THREADS) {
             if (reload_p) S.P[i] = __ldg(th + i);
-            S.V[i] = __ldcg(vg + i);                             // written by the previous kernel on this stream
+            const float v = __ldcg(vg + i);                      // written by the previous kernel on this stream
+            S.V[i] = A.step_size ? __ldg(A.step_size + i) * v : v;       // the direction H is applied to: alpha * vec
         }
         __syncthreads();
         for (int i = tid; i < HID * HID; i += PT_THREADS) {
@@ -1509,6 +1510,7 @@ static int chain_stage_args(const promp_policy_stage* stages, int n_stages, int 
         a.ls_per_sample = g.ls_per_sample; a.obj_kind = g.obj_kind; a.kl_coeff = g.kl_coeff;
         a.clip_log_std = g.clip_log_std; a.min_log_std = min_log_std; a.stats = g.stats; a.n_valid = g.n_valid;
         a.kl_coeff_ptr = g.kl_coeff_dev;
+        a.step_size = g.step_size;
         if (g.kind == 0) {
             PROMP_REQUIRE(g.obj_kind >= 0 && g.obj_kind <= PROMP_OBJ_EXPLORE, "promp_policy_chain: stage %d: bad obj_kind %d", s,
                           g.obj_kind);

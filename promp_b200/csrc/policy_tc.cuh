@@ -789,8 +789,19 @@ __device__ __forceinline__ void hvp_tc_tiles(const PolicyArgs& A, HvpTcSmem<DO, 
     // The direction vector may be read through the read-only path only if nothing in this launch writes it: out != vec (the
     // in-place form v <- v - alpha H v rewrites task m's slice at its flush) and no producer stage in the same launch.
     const bool vec_ro = A.out != A.vec;
-    auto ldv = [&](const float* p) { return vec_ro ? Sched::ldp(p) : __ldcg(p); };
-    auto ldv4 = [&](const float4* p) { return vec_ro ? Sched::ldp4(p) : __ldcg(p); };
+    // Per-parameter step sizes (A.step_size): H is applied to alpha * vec, so every staged direction element i - both the
+    // shared-memory copy and the W1 weight buffers - is scaled by alpha[i]; the epilogue's vec stays unscaled.
+    const float* const al = A.step_size;
+    auto ldv = [&](const float* p) {
+        const float v = vec_ro ? Sched::ldp(p) : __ldcg(p);
+        return al ? __ldg(al + (p - vg)) * v : v;
+    };
+    auto ldv4 = [&](const float4* p) {
+        const float4 v = vec_ro ? Sched::ldp4(p) : __ldcg(p);
+        if (!al) return v;
+        const float4 a = __ldg(reinterpret_cast<const float4*>(al + (reinterpret_cast<const float*>(p) - vg)));
+        return make_float4(a.x * v.x, a.y * v.y, a.z * v.z, a.w * v.w);
+    };
     auto load_task = [&](int m) {
         sc.wait_task(m);
         if (A.n_valid) { Nm = __ldg(A.n_valid + m); invN = 1.0f / (float)max(Nm, 1); }

@@ -10,6 +10,12 @@ differentiate through the inner SGD step.  Here the same quantities are produced
 
 which is exactly d/dtheta of the meta objective for any number of inner steps (the backward chain
 is the transpose of d theta_{s+1} / d theta_s = I - alpha H_s).
+
+trainable_inner_step_size=True (Meta-SGD, Li et al. 2017; ref base.py:98, 210, 303-313): alpha is a vector [P] in the
+policy's device layout, shared by every task and inner step, that starts at inner_lr and is trained with theta:
+  forward chain   theta_{s+1,i} = theta_{s,i} - alpha * g_{s,i}                      (alpha: PolicyStage.step_size)
+  backward chain  v_i <- v_i - H_s,i (alpha * v_i) + c_s * grad KL_s,i
+  alpha gradient  -(1/M) sum_i sum_s v_{s+1,i} * g_{s,i}   (v_{s+1,i}: the vector entering the HVP stage of step s)
 """
 import ctypes
 import os
@@ -25,7 +31,7 @@ class MAMLAlgo(object):
     """
     Args:
         policy (MetaGaussianMLPPolicy), inner_lr, meta_batch_size, num_inner_grad_steps,
-        trainable_inner_step_size (must be False, as in every shipped reference config)
+        trainable_inner_step_size (bool): learn one inner step size per policy parameter (Meta-SGD) with the outer optimizer
     """
     inner_obj_kind = _lib.OBJ_RATIO
     CHAIN_MAX_STAGES = 6          # promp_policy_chain's stage limit
@@ -41,20 +47,30 @@ class MAMLAlgo(object):
                              "KL-coefficient kernels take up to %d sampling phases)"
                              % (num_inner_grad_steps, self.MAX_INNER_GRAD_STEPS, self.MAX_INNER_GRAD_STEPS + 1))
         assert type(meta_batch_size) == int
-        if trainable_inner_step_size:
-            raise NotImplementedError("trainable_inner_step_size is not supported (reference: 'it isn't supported "
-                                      "right now', meta_algos/base.py:203)")
         self.policy = policy
         self.inner_lr = float(inner_lr)
         self.meta_batch_size = meta_batch_size
         self.num_inner_grad_steps = num_inner_grad_steps
-        self.trainable_inner_step_size = trainable_inner_step_size
+        self.trainable_inner_step_size = bool(trainable_inner_step_size)
+        # alpha [P] on the device (padded layout included), trained by the outer optimizer; None = the scalar inner_lr
+        self.alpha = None
+        if self.trainable_inner_step_size:
+            import torch
+            self.alpha = torch.full((policy.num_params,), self.inner_lr, dtype=torch.float32, device=policy.device)
         self._optimization_keys = None
         self._ws = None
         self._ws_chain = None
         self._stats_ring = {}
         # the gradient chain of a meta-objective evaluation as ONE dataflow launch (promp_policy_chain) or as one launch per stage
         self.use_chain = os.environ.get('PROMP_B200_CHAIN', '1') != '0'
+
+    @property
+    def step_sizes(self):
+        """The inner step sizes as the reference's `step_sizes` dict: parameter key -> numpy array of the parameter's shape
+        (inner_lr everywhere unless trainable_inner_step_size)."""
+        p = self.policy
+        flat = self.alpha.cpu().numpy() if self.alpha is not None else np.full(p.num_params, self.inner_lr, np.float32)
+        return p._unflatten_np(p.unpad_flat(flat).copy())
 
     # ------------------------------------------------------------------------------------ helpers
     def _workspace(self, N):
@@ -128,7 +144,8 @@ class MAMLAlgo(object):
 
     def _stage(self, kind, phase, params, stride, obj_kind, obj_scale=1.0, clip_eps=0.0, kl_coeff=0.0, clip_log_std=0, grad=None,
                out_params=None, sgd_lr=0.0, vec=None, out=None, stats=None, kl_coeff_dev=None, adv=None):
-        """One promp_policy_stage (kind 0: the arguments of _grad, kind 1: those of _hvp)."""
+        """One promp_policy_stage (kind 0: the arguments of _grad, kind 1: those of _hvp).  With trainable step sizes, the SGD
+        step of a gradient stage with out_params and every HVP stage use alpha (self.alpha) in place of inner_lr."""
         full = getattr(phase, 'log_std_full', None)
         old_ls, per_sample = (full, 1) if full is not None else (phase.log_std, 0)
         st = _lib.PolicyStage()
@@ -142,6 +159,9 @@ class MAMLAlgo(object):
         st.grad, st.out_params, st.sgd_lr = _lib.ptr(grad), _lib.ptr(out_params), float(sgd_lr)
         st.inner_lr, st.vec, st.out, st.stats = float(self.inner_lr), _lib.ptr(vec), _lib.ptr(out), _lib.ptr(stats)
         st.kl_coeff_dev = _lib.ptr(kl_coeff_dev)      # optional device-resident multiplier of kl_coeff
+        if self.alpha is not None and (kind == 1 or out_params is not None):
+            st.step_size = _lib.ptr(self.alpha)
+            st.inner_lr = 1.0                          # HVP stage: vec - H (alpha * vec)
         return st
 
     def _run_chain(self, stages, reuse=None):
@@ -195,6 +215,13 @@ class MAMLAlgo(object):
         new = torch.empty(M, P, dtype=torch.float32, device=p.device)
         produce, stats = None, None
         self._adapt_cache = None
+        if self.alpha is not None:
+            # per-parameter step sizes go through the stage path; no launch re-use (the first Adam epoch recomputes stage 0)
+            st = self._stage(0, phase, params, stride, self.inner_obj_kind, grad=grad, out_params=new)
+            self._run_chain([st])
+            self.last_inner_grad = grad
+            p.update_task_parameters(new)
+            return
         if stride == 0 and params is p.theta and getattr(phase, 'n_valid', None) is None:
             if getattr(self, '_reuse_bufs', None) is None:
                 self._reuse_bufs = (torch.zeros(1, dtype=torch.int32, device=p.device),
@@ -228,6 +255,9 @@ class MAMLAlgo(object):
                      surr=[M] outer surrogate per task, outer_kl=[M], inner_kl=[S-1, M]).
         reduce=False leaves the per-task gradients in out['grad_tasks'] [M, P] for the fused reduce + all-reduce + Adam
         kernel (promp_meta_update) and skips promp_reduce_tasks.
+        Trainable step sizes: out['sgd_pairs'] = [(v_{s+1}, g_s)] per inner step s (the direction entering HVP stage s and the
+        inner gradient of stage s, both [M, P]) for promp_meta_update_sgd, and with reduce=True out['grad'] is the [2P]
+        gradient [theta; alpha].
         explore: the E-MAML coefficient c [M] (device) or None.  The exploration term -c_m * mean logp_theta(a|x) on the
         phase-0 data (trpo_maml.py:137-144) is then one more gradient stage (OBJ_EXPLORE at theta, clipped log_std) of the
         chain; out['explore'] = its value per task [M], and its gradient is summed into out['grad'] by the same reduction."""
@@ -240,7 +270,11 @@ class MAMLAlgo(object):
         x_grad = torch.empty(M, P, dtype=torch.float32, device=dev) if explore is not None and want_grad else None
 
         def reduced(v):
-            flat = torch.empty(P, dtype=torch.float32, device=dev)
+            flat = torch.empty(P if self.alpha is None else 2 * P, dtype=torch.float32, device=dev)
+            if self.alpha is not None:       # the alpha half first (task_grads NULL: promp_reduce_tasks_sgd writes only it)
+                lam, g = _lib.ptr_array([a for a, _ in pairs]), _lib.ptr_array([b for _, b in pairs])   # kept alive here
+                _lib.call('promp_reduce_tasks_sgd', M, P, None, len(pairs), lam, g, 1.0 / (M * world_size()), _lib.ptr(flat),
+                          _lib.stream())
             if x_grad is None:
                 _lib.call('promp_reduce_tasks', M, P, _lib.ptr(v), 1.0 / (M * world_size()), _lib.ptr(flat), _lib.stream())
             else:
@@ -252,6 +286,8 @@ class MAMLAlgo(object):
             self._grad(phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=x_grad, stats=x_stats, adv=explore)
         cur, stride, clip = theta, 0, 1              # step 0 = distribution_info_sym(params=None): clipped log_std
         chain = []
+        pairs = []                                   # trainable step sizes: (v_{s+1}, g_s) per inner step
+        trainable = self.alpha is not None
         # The inner pass at step 0 repeats the _adapt launch as long as theta has not been updated since (first Adam epoch,
         # "loss before" passes): aim it at the SAME output buffers and let the kernel skip itself after verifying on the
         # device that the parameters are bit-identical and the step-0 log_std clip is inactive.  Host-side conditions: same
@@ -271,7 +307,7 @@ class MAMLAlgo(object):
             host = inner_kl_coeffs_dev.cpu().numpy()
             inner_kl_coeffs = [float(np.float32(sc) * np.float32(c)) for sc, c in zip(inner_kl_coeffs, host)]
             inner_kl_coeffs_dev = None
-        if self.use_chain and (S >= 2 or want_grad):
+        if (self.use_chain or trainable) and (S >= 2 or want_grad):
             # the whole chain - inner gradients + SGD steps, outer gradient, backward Hessian-vector chain - as ONE launch
             stages = []
             for s in range(S - 1):
@@ -296,14 +332,22 @@ class MAMLAlgo(object):
                                               clip_log_std=clp, vec=v, out=v_out,
                                               kl_coeff_dev=None if inner_kl_coeffs_dev is None else inner_kl_coeffs_dev[s:s + 1]))
                     chain.append(v)       # the stage list holds raw pointers: keep every buffer alive until the launch is enqueued
+                    if trainable:
+                        pairs.insert(0, (v, chain[s][3]))
                     v = v_out
             if explore is not None:
                 # last stage, waits for no other: in the dataflow kernel it fills the tail of the backward chain
                 stages.append(self._stage(0, phases[0], theta, 0, _lib.OBJ_EXPLORE, clip_log_std=1, grad=x_grad, stats=x_stats,
                                           adv=explore))
-            self._run_chain(stages, reuse=self._reuse_bufs if reuse0 else None)
+            if trainable and not self.use_chain:
+                for st in stages:                      # one launch per stage
+                    self._run_chain([st])
+            else:
+                self._run_chain(stages, reuse=self._reuse_bufs if reuse0 else None)
             out = dict(surr=stats_all[S - 1, :, 0], outer_kl=stats_all[S - 1, :, 1], inner_kl=stats_all[:S - 1, :, 1],
                        stats_all=stats_all, grad=None)
+            if trainable and want_grad:
+                out['sgd_pairs'] = pairs
             if x_stats is not None:
                 out['explore'] = x_stats[:, 0]
             if want_grad:

@@ -28,7 +28,7 @@ class ProMP(MAMLAlgo):
         self.name = name
         self.kl_coeff = [init_inner_kl_penalty] * self.meta_batch_size * self.num_inner_grad_steps
         self.inner_obj_kind = _lib.OBJ_RATIO                     # _adapt_objective_sym (pro_mp.py:59-65)
-        self.optimizer.build(self.policy)
+        self.optimizer.build(self.policy, alpha=self.alpha)
 
     FUSED_META_UPDATE = True     # _objective_pass(reduce=False) -> per-task gradients for promp_meta_update
 

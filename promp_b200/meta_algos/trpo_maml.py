@@ -13,6 +13,10 @@ class TRPOMAML(MAMLAlgo):
 
     def __init__(self, *args, name="trpo_maml", step_size=0.01, inner_type='likelihood_ratio', exploration=False,
                  **kwargs):
+        if kwargs.get('trainable_inner_step_size', len(args) > 4 and args[4]):
+            raise NotImplementedError("TRPOMAML does not support trainable_inner_step_size: the KL trust region has no curvature "
+                                      "along the inner step sizes, so conjugate gradient over [theta; alpha] is singular "
+                                      "(ProMP and VPGMAML support it)")
         super(TRPOMAML, self).__init__(*args, **kwargs)
         assert inner_type in ["log_likelihood", "likelihood_ratio", "dice"]
         if inner_type == 'dice':

@@ -26,7 +26,7 @@ class VPGMAML(MAMLAlgo):
         if exploration:
             self._optimization_keys.append('adj_avg_rewards')
         self.inner_obj_kind = _lib.OBJ_RATIO if inner_type == 'likelihood_ratio' else _lib.OBJ_LOGLIK
-        self.optimizer.build(self.policy)
+        self.optimizer.build(self.policy, alpha=self.alpha)
 
     # the E-MAML term is shared with TRPOMAML (same formula, vpg_maml.py:137-144 == trpo_maml.py:137-144).  The Trainer never
     # captures VPGMAML into a CUDA graph (it has no optimize_phases); its coefficient is device-side all the same.

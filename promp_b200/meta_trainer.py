@@ -149,13 +149,14 @@ class Trainer(object):
         # The warm-up passes below are REAL meta-iterations (they size the allocator pools and JIT nothing, but they do train
         # the policy and consume random numbers).  Everything they touch is saved here and put back after the capture, so
         # that step(0) is the run's first iteration exactly as in eager mode: parameters, Adam slots, the device Philox phase
-        # counter, the global numpy stream.
+        # counter, the global numpy stream; with trainable inner step sizes also alpha and its Adam slots.
         opt = getattr(algo, 'optimizer', None)
+        alpha = getattr(algo, 'alpha', None)
         torch.cuda.synchronize()
-        saved = dict(theta=policy.theta.clone(), np_state=np.random.get_state(),
+        saved = dict(theta=policy.theta.clone(), alpha=alpha.clone() if alpha is not None else None, np_state=np.random.get_state(),
                      kl_coeff=np.array(algo.inner_kl_coeff, dtype=np.float64) if hasattr(algo, 'inner_kl_coeff') else None,
                      phase_counter_dev=sampler._phase_counter_dev.clone(),
-                     adam=[t.clone() for t in (opt.m, opt.v, opt.step)] if hasattr(opt, 'm') else None)
+                     adam=[t.clone() for t in opt.slots()] if hasattr(opt, 'slots') else None)
         if log:
             n_env_keys = len(getattr(inner_env, 'DEVICE_LOG_KEYS', ()))
             n_log = S * (7 + n_env_keys) + len(algo.LOG_KEYS)
@@ -188,8 +189,10 @@ class Trainer(object):
             if gc_was_enabled:
                 gc.enable()
         policy.theta.copy_(saved['theta'])
+        if alpha is not None:
+            alpha.copy_(saved['alpha'])
         if saved['adam'] is not None:
-            for dst, src in zip((opt.m, opt.v, opt.step), saved['adam']):
+            for dst, src in zip(opt.slots(), saved['adam']):
                 dst.copy_(src)
         sampler._phase_counter_dev.copy_(saved['phase_counter_dev'])
         if saved['kl_coeff'] is not None:
@@ -278,7 +281,7 @@ class Trainer(object):
     def get_itr_snapshot(self, itr):
         """meta_trainer.py:153-158: {itr, policy, env, baseline} (picklable: the policy pickles its init arguments and a
         host copy of the parameters, policies/base.py:205-215), plus what a bit-identical resume needs and the reference
-        drops: optimizer slots, adaptive KL coefficients, the sampled-timesteps counter."""
+        drops: optimizer slots, adaptive KL coefficients, the sampled-timesteps counter, trainable inner step sizes."""
         snap = dict(itr=itr, policy=self.policy, env=self.env, baseline=self.baseline)
         extra = dict(total_timesteps_sampled=self.sampler.total_timesteps_sampled)
         opt = getattr(self.algo, 'optimizer', None)
@@ -286,6 +289,8 @@ class Trainer(object):
             extra['optimizer'] = opt.get_state()
         if hasattr(self.algo, 'inner_kl_coeff'):
             extra['inner_kl_coeff'] = np.asarray(self.algo.inner_kl_coeff, dtype=np.float64).copy()
+        if getattr(self.algo, 'alpha', None) is not None:
+            extra['alpha'] = self.algo.alpha.cpu().numpy()
         snap['promp_b200_state'] = extra
         return snap
 
@@ -302,6 +307,9 @@ class Trainer(object):
         opt = getattr(self.algo, 'optimizer', None)
         if 'optimizer' in extra and hasattr(opt, 'set_state'):
             opt.set_state(extra['optimizer'])
+        if 'alpha' in extra and getattr(self.algo, 'alpha', None) is not None:
+            import torch
+            self.algo.alpha.copy_(torch.from_numpy(extra['alpha']))
         if 'inner_kl_coeff' in extra and hasattr(self.algo, 'inner_kl_coeff'):
             self.algo.inner_kl_coeff = np.asarray(extra['inner_kl_coeff'], dtype=np.float64).copy()
         self.sampler.total_timesteps_sampled = int(extra.get('total_timesteps_sampled', self.sampler.total_timesteps_sampled))
