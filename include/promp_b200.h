@@ -71,6 +71,17 @@ enum {
  * PROMP_OUT_TANH), at width 32 or 64, and does not change the layout or the workspace sizes either.  Bits 0x200 - 0x800
  * stay unknown (rejected). */
 #define PROMP_OUT_TANH 0x1000
+/* Number of hidden layers (policies/networks/mlp.py: len(hidden_sizes)), in the same `hidden` argument: a 3-bit field at
+ * PROMP_HIDDEN_DEPTH_SHIFT.  No depth bits = two hidden layers, so every value above keeps its meaning; PROMP_HIDDEN_DEPTH(1)
+ * and PROMP_HIDDEN_DEPTH(3) select one and three hidden layers of the same width (32 or 64), with any activation flags.
+ * Field values 4..7 are rejected.  The depth changes the layout: a depth-L parameter vector is
+ *   W0[Do,Hd] b0[Hd] {W_l[Hd,Hd] b_l[Hd]}_{l=1..L-1} W_out[Hd,Da] b_out[Da] log_std[Da]
+ * (the reference's creation order: hidden_0 .. hidden_{L-1}, output, log_std), and promp_num_params, promp_policy_layout and
+ * the workspace sizes count it.  Policies of depth 1 and 3 run CUDA-core kernels of their own; the chain entry point runs
+ * their stages as one launch each. */
+#define PROMP_HIDDEN_DEPTH_SHIFT 14
+#define PROMP_HIDDEN_DEPTH_MASK 0x1C000
+#define PROMP_HIDDEN_DEPTH(layers) ((layers) << PROMP_HIDDEN_DEPTH_SHIFT)
 /* baseline kinds of promp_process_samples.  LINEAR_TIME (baselines/linear_baseline.py:109-126) fits [t, t^2, t^3, 1],
  * t = step / 100, and never reads obs; its coefficients are [M,4].  GIVEN: the caller supplies the per-sample baseline
  * values (promp_process_samples_given); no fit, no coefficients. */
@@ -79,7 +90,7 @@ enum { PROMP_BASELINE_ZERO = 0, PROMP_BASELINE_LINEAR_FEATURE = 1, PROMP_BASELIN
 const char* promp_last_error(void);
 int promp_version(void);
 
-/* Number of policy parameters P for (obs_dim, act_dim, hidden,hidden). */
+/* Number of policy parameters P for (obs_dim, act_dim, hidden,hidden), or for the depth the `hidden` argument carries. */
 int promp_num_params(int obs_dim, int act_dim, int hidden);
 /* State floats per env for init_state / final_state: 2 (point envs; 4 = pos, vel for the momentum env), 18 (cheetah, walker:
  * qpos[9] qvel[9]), 10 (swimmer: qpos[5] qvel[5]). */
@@ -228,7 +239,8 @@ int promp_paths_histogram(int M, int E, int timeline_len, const uint8_t* t_done,
  * promp_env_module_load: loads the cubin `image` (`bytes` long) and resolves its kernels by their lowered names.
  *   names [PROMP_ENV_MODULE_SLOTS]: slot PROMP_ENV_SLOT_STEP = env_step_kernel, PROMP_ENV_SLOT_OBSERVE = env_observe_kernel,
  *   PROMP_ENV_SLOT_ROLLOUT + 2*v + keyed = rollout_kernel of `hidden` variant v = (relu + 2*out_tanh)*2 + (width == 64),
- *   keyed = the sharded (task_offset != 0) instantiation.  NULL or "" = not compiled; launching it returns
+ *   keyed = the sharded (task_offset != 0) instantiation; PROMP_ENV_SLOT_ROLLOUT_DEEP + 2*v + keyed = rollout_deep_kernel, the
+ *   same variants at depth 1 or 3 (PROMP_HIDDEN_DEPTH).  NULL or "" = not compiled; launching it returns
  *   PROMP_ERR_INVALID_ARG.  dims [PROMP_ENV_MODULE_NDIMS] = {obs, act, state, task sizes, info channels, ends early}; obs
  *   1..19, act 1..8 (the rollout policy's range), info 0..3.  *handle_out: the module, until promp_env_module_unload.
  *   There is no reference counterpart (the reference steps Python envs, envs/base.py:6-49).
@@ -241,11 +253,12 @@ int promp_paths_histogram(int M, int E, int timeline_len, const uint8_t* t_done,
  * promp_env_step_module / promp_env_observe_module: promp_env_step / promp_env_observe (MetaIterativeEnvExecutor.step /
  *   reset, vectorized_env_executor.py:25-75) for the module's env; info [NINFO, n_env] or NULL.
  */
-#define PROMP_ENV_MODULE_SLOTS 18
+#define PROMP_ENV_MODULE_SLOTS 34
 #define PROMP_ENV_MODULE_NDIMS 6
 #define PROMP_ENV_SLOT_STEP 0
 #define PROMP_ENV_SLOT_OBSERVE 1
 #define PROMP_ENV_SLOT_ROLLOUT 2
+#define PROMP_ENV_SLOT_ROLLOUT_DEEP 18
 int promp_env_module_load(const void* image, int64_t bytes, const char* const* names, int n_names, const int* dims,
                           void** handle_out);
 int promp_env_module_unload(void* handle);

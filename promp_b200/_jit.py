@@ -45,23 +45,33 @@ class CudaEnvCompileError(RuntimeError):
 
 
 # ---------------------------------------------------------------------------------------------------------- names
-def rollout_slot(hidden, keyed):
-    """Kernel slot of the rollout kernel of a `hidden` argument (width | ACT_RELU | OUT_TANH), as env_module.cu."""
+def _variant(hidden):
+    """(v, deep) of a `hidden` argument (width | ACT_RELU | OUT_TANH | depth bits): v = the variant index of env_module.cu,
+    deep = one or three hidden layers (rollout_deep_kernel)."""
     width, relu, otanh = hidden & _lib.HIDDEN_WIDTH_MASK, bool(hidden & _lib.ACT_RELU), bool(hidden & _lib.OUT_TANH)
-    if width not in (32, 64) or hidden & ~(_lib.HIDDEN_WIDTH_MASK | _lib.ACT_RELU | _lib.OUT_TANH):
-        raise ValueError("user envs run policies of hidden width 32 or 64 (hidden argument 0x%x)" % hidden)
-    v = (int(relu) + 2 * int(otanh)) * 2 + int(width == 64)
-    return _lib.ENV_SLOT_ROLLOUT + 2 * v + int(keyed)
+    depth = (hidden & _lib.HIDDEN_DEPTH_MASK) >> _lib.HIDDEN_DEPTH_SHIFT
+    known = _lib.HIDDEN_WIDTH_MASK | _lib.ACT_RELU | _lib.OUT_TANH | _lib.HIDDEN_DEPTH_MASK
+    if width not in (32, 64) or hidden & ~known or depth > 3:
+        raise ValueError("user envs run policies of hidden width 32 or 64 and 1 to 3 hidden layers (hidden argument 0x%x)"
+                         % hidden)
+    return (int(relu) + 2 * int(otanh)) * 2 + int(width == 64), depth not in (0, 2)
+
+
+def rollout_slot(hidden, keyed):
+    """Kernel slot of the rollout kernel of a `hidden` argument, as env_module.cu."""
+    v, deep = _variant(hidden)
+    return (_lib.ENV_SLOT_ROLLOUT_DEEP if deep else _lib.ENV_SLOT_ROLLOUT) + 2 * v + int(keyed)
 
 
 def name_expressions(hiddens=()):
     """{slot: name expression}: the env-step and env-observe kernels, and both rollout kernels of every `hidden`."""
     out = {_lib.ENV_SLOT_STEP: 'promp::env_step_kernel<%s>' % ENV, _lib.ENV_SLOT_OBSERVE: 'promp::env_observe_kernel<%s>' % ENV}
     for h in hiddens:
-        act = ACTS[(rollout_slot(h, False) - _lib.ENV_SLOT_ROLLOUT) // 4]
+        v, deep = _variant(h)
         for keyed in (False, True):
-            out[rollout_slot(h, keyed)] = 'promp::rollout_kernel<%s, %d, %s, %s>' % (
-                ENV, h & _lib.HIDDEN_WIDTH_MASK, act, 'true' if keyed else 'false')
+            out[rollout_slot(h, keyed)] = 'promp::%s<%s, %d, %s, %s>' % (
+                'rollout_deep_kernel' if deep else 'rollout_kernel', ENV, h & _lib.HIDDEN_WIDTH_MASK, ACTS[v // 2],
+                'true' if keyed else 'false')
     return out
 
 

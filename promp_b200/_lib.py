@@ -17,12 +17,20 @@ ENV_WALKER, ENV_SWIMMER = 5, 6
 EARLY_TERM_ENVS = (ENV_POINT, ENV_WALKER)        # env kinds whose paths end on `done` (variable-length paths)
 INFO_ENVS = (ENV_CHEETAH_DIR, ENV_SWIMMER)       # env kinds whose kernels write env_infos channels
 # env modules (promp_env_module_load): kernel slots and dims
-ENV_MODULE_SLOTS, ENV_MODULE_NDIMS, ENV_SLOT_STEP, ENV_SLOT_OBSERVE, ENV_SLOT_ROLLOUT = 18, 6, 0, 1, 2
+ENV_MODULE_SLOTS, ENV_MODULE_NDIMS, ENV_SLOT_STEP, ENV_SLOT_OBSERVE, ENV_SLOT_ROLLOUT = 34, 6, 0, 1, 2
+ENV_SLOT_ROLLOUT_DEEP = 18
 REWARD_SPARSE, REWARD_DENSE, REWARD_DENSE_SQUARED = 0, 1, 2
 OBJ_RATIO, OBJ_LOGLIK, OBJ_CLIP, OBJ_NONE, OBJ_EXPLORE = 0, 1, 2, 3, 4
 BASELINE_ZERO, BASELINE_LINEAR_FEATURE, BASELINE_LINEAR_TIME, BASELINE_GIVEN = 0, 1, 2, 3
 # the policy / rollout `hidden` argument: width | activation flag (no flag = tanh) | output flag (no flag = identity)
 HIDDEN_WIDTH_MASK, ACT_RELU, OUT_TANH = 0xFF, 0x100, 0x1000
+# ... | the number of hidden layers in a 3-bit field (no bits = two hidden layers)
+HIDDEN_DEPTH_SHIFT, HIDDEN_DEPTH_MASK = 14, 0x1C000
+
+
+def hidden_depth(layers):
+    """The depth bits of the `hidden` argument for `layers` hidden layers (PROMP_HIDDEN_DEPTH; 0 for two layers)."""
+    return 0 if layers == 2 else layers << HIDDEN_DEPTH_SHIFT
 
 _P = c_void_p
 

@@ -59,6 +59,22 @@ struct PLayout {
 __host__ __device__ inline int num_params(int Do, int Da, int Hd) {
     return Do * Hd + Hd + Hd * Hd + Hd + Hd * Da + Da + Da;
 }
+// Any depth (1..3 hidden layers): W0[Do,Hd] b0[Hd] {W_l[Hd,Hd] b_l[Hd]}_{l=1..depth-1} W_out[Hd,Da] b_out[Da] log_std[Da]
+__host__ __device__ inline int num_params(int Do, int Da, int Hd, int depth) {
+    return Do * Hd + Hd + (depth - 1) * (Hd * Hd + Hd) + Hd * Da + Da + Da;
+}
+// The same layout with the number of hidden-to-hidden layers nh = depth - 1 known at run time (the kernels of depth 1 and 3)
+template <int DO, int DA, int HID>
+struct DeepLayout {
+    int nh;
+    static constexpr int W0 = 0, B0 = DO * HID;
+    __host__ __device__ int wh(int l) const { return B0 + HID + l * (HID * HID + HID); }   // W_{l+1}, l < nh
+    __host__ __device__ int bh(int l) const { return wh(l) + HID * HID; }
+    __host__ __device__ int wo() const { return wh(nh); }
+    __host__ __device__ int bo() const { return wo() + HID * DA; }
+    __host__ __device__ int ls() const { return bo() + DA; }
+    __host__ __device__ int P() const { return ls() + DA; }
+};
 
 // ---------------------------------------------------------------- math
 // tanh via one ex2.approx + one fast division: |abs error| <= ~2e-7 over the whole range (saturates to +-1
@@ -159,18 +175,25 @@ __device__ __forceinline__ void out_hvp_back(const float (&mu)[DA], const float 
 
 #ifndef __CUDACC_RTC__
 // The `hidden` argument of the policy and rollout entry points: the width (32 or 64) in the low byte, PROMP_ACT_RELU and
-// PROMP_OUT_TANH above it.  A plain width selects tanh hidden layers and the identity output.
-inline int decode_hidden(const char* who, int hidden, int& width, bool& relu, bool& out_tanh) {
-    constexpr int known = PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU | PROMP_OUT_TANH;
+// PROMP_OUT_TANH above it, the number of hidden layers in the PROMP_HIDDEN_DEPTH_MASK field (no bits = 2).  A plain width
+// selects two tanh hidden layers and the identity output.
+inline int decode_hidden(const char* who, int hidden, int& width, bool& relu, bool& out_tanh, int& depth) {
+    constexpr int known = PROMP_HIDDEN_WIDTH_MASK | PROMP_ACT_RELU | PROMP_OUT_TANH | PROMP_HIDDEN_DEPTH_MASK;
     PROMP_REQUIRE((hidden & ~known) == 0,
-                  "%s: unknown flag bits 0x%x in hidden (%d); known: PROMP_ACT_RELU = 0x%x, PROMP_OUT_TANH = 0x%x", who,
-                  hidden & ~known, hidden, PROMP_ACT_RELU, PROMP_OUT_TANH);
+                  "%s: unknown flag bits 0x%x in hidden (%d); known: PROMP_ACT_RELU = 0x%x, PROMP_OUT_TANH = 0x%x, "
+                  "PROMP_HIDDEN_DEPTH_MASK = 0x%x", who, hidden & ~known, hidden, PROMP_ACT_RELU, PROMP_OUT_TANH,
+                  PROMP_HIDDEN_DEPTH_MASK);
     width = hidden & PROMP_HIDDEN_WIDTH_MASK;
     relu = (hidden & PROMP_ACT_RELU) != 0;
     out_tanh = (hidden & PROMP_OUT_TANH) != 0;
+    const int field = (hidden & PROMP_HIDDEN_DEPTH_MASK) >> PROMP_HIDDEN_DEPTH_SHIFT;
+    depth = field == 0 ? 2 : field;
     PROMP_REQUIRE(!relu || width == 32 || width == 64, "%s: ReLU policies are built for hidden 32 or 64 (got %d)", who, width);
     PROMP_REQUIRE(!out_tanh || width == 32 || width == 64, "%s: tanh-output policies are built for hidden 32 or 64 (got %d)",
                   who, width);
+    PROMP_REQUIRE(depth <= 3, "%s: policies have 1 to 3 hidden layers (depth field %d in hidden 0x%x)", who, depth, hidden);
+    PROMP_REQUIRE(field == 0 || width == 32 || width == 64,
+                  "%s: policies of depth 1 or 3 are built for hidden 32 or 64 (got %d)", who, width);
     return PROMP_OK;
 }
 

@@ -12,10 +12,11 @@ struct EnvModule {
     int dims[PROMP_ENV_MODULE_NDIMS];
 };
 
-// slot of the rollout kernel of one `hidden` variant (decode_hidden), keyed (sharded launch) or not
-static int rollout_slot(bool relu, bool out_tanh, int width, bool keyed) {
+// slot of the rollout kernel of one `hidden` variant (decode_hidden), keyed (sharded launch) or not; depth 1 and 3 share the
+// rollout_deep_kernel slots
+static int rollout_slot(bool relu, bool out_tanh, int width, bool keyed, int depth) {
     const int v = ((relu ? 1 : 0) + (out_tanh ? 2 : 0)) * 2 + (width == 64 ? 1 : 0);
-    return PROMP_ENV_SLOT_ROLLOUT + 2 * v + (keyed ? 1 : 0);
+    return (depth == 2 ? PROMP_ENV_SLOT_ROLLOUT : PROMP_ENV_SLOT_ROLLOUT_DEEP) + 2 * v + (keyed ? 1 : 0);
 }
 
 static EnvModule* as_module(const char* fn, void* h) {
@@ -23,10 +24,10 @@ static EnvModule* as_module(const char* fn, void* h) {
     return (EnvModule*)h;
 }
 
-static int launch(const char* fn, EnvModule* m, int slot, dim3 grid, dim3 block, void** args, cudaStream_t st) {
+static int launch(const char* fn, EnvModule* m, int slot, dim3 grid, dim3 block, void** args, int smem, cudaStream_t st) {
     PROMP_REQUIRE(m->k[slot] != nullptr, "%s: kernel slot %d was not compiled into this env module (the policy's hidden "
                                          "variant or the env kernels were not requested)", fn, slot);
-    PROMP_CUDA(cudaLaunchKernel((const void*)m->k[slot], grid, block, args, 0, st));
+    PROMP_CUDA(cudaLaunchKernel((const void*)m->k[slot], grid, block, args, smem, st));
     return PROMP_OK;
 }
 
@@ -43,9 +44,9 @@ static int rollout_module(const char* fn, void* handle, int reward_type, float r
     PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
     if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
-    int width;
+    int width, depth;
     bool relu, out_tanh;
-    if (decode_hidden(fn, hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    if (decode_hidden(fn, hidden, width, relu, out_tanh, depth) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
     PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "%s: bad reward_type %d", fn, reward_type);
     const int ninfo = m->dims[4], ends_early = m->dims[5];
@@ -59,9 +60,11 @@ static int rollout_module(const char* fn, void* handle, int reward_type, float r
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done,
                   early_term ? nullptr : info, log_std_out, early_term ? nullptr : final_state, early_term, horizon,
                   (uint32_t)task_offset * (uint32_t)E};
-    void* args[] = {&A};
+    int nh = depth - 1;
+    void* args[] = {&A, &nh};
     const dim3 grid((E + RO_WARPS - 1) / RO_WARPS, M);
-    return launch(fn, m, rollout_slot(relu, out_tanh, width, A.key_offset != 0), grid, dim3(RO_WARPS * 32), args,
+    const int smem = depth == 2 ? 0 : (width == 64 ? rollout_deep_smem_bytes<64>(nh) : rollout_deep_smem_bytes<32>(nh));
+    return launch(fn, m, rollout_slot(relu, out_tanh, width, A.key_offset != 0, depth), grid, dim3(RO_WARPS * 32), args, smem,
                   (cudaStream_t)stream);
 }
 
@@ -93,6 +96,15 @@ extern "C" int promp_env_module_load(const void* image, int64_t bytes, const cha
             cudaLibraryUnload(m->lib);
             delete m;
             return check_cuda(ek, names[i]);
+        }
+        if (i >= PROMP_ENV_SLOT_ROLLOUT_DEEP) {      // rollout_deep_kernel: hidden layers in dynamic shared memory (> 48 KB)
+            const int smem = ((i - PROMP_ENV_SLOT_ROLLOUT_DEEP) / 2) % 2 ? rollout_deep_smem_bytes<64>(2) : rollout_deep_smem_bytes<32>(2);
+            const cudaError_t ea = cudaFuncSetAttribute((const void*)m->k[i], cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            if (ea != cudaSuccess) {
+                cudaLibraryUnload(m->lib);
+                delete m;
+                return check_cuda(ea, "cudaFuncSetAttribute (rollout_deep_kernel)");
+            }
         }
     }
     *handle_out = m;
@@ -144,7 +156,7 @@ extern "C" int promp_env_step_module(void* module, int reward_type, float sparse
     EnvCfg cfg{reward_type, sparse_radius, normalize_actions != 0};
     void* args[] = {&cfg, &n_env, &H, &state, &ts, &actions, &task_params, &reset_state, &next_obs, &rew, &done, &info};
     const int bs = 128;
-    return launch(fn, m, PROMP_ENV_SLOT_STEP, dim3((n_env + bs - 1) / bs), dim3(bs), args, (cudaStream_t)stream);
+    return launch(fn, m, PROMP_ENV_SLOT_STEP, dim3((n_env + bs - 1) / bs), dim3(bs), args, 0, (cudaStream_t)stream);
 }
 
 extern "C" int promp_env_observe_module(void* module, int n_env, const float* state, float* obs, void* stream) {
@@ -154,7 +166,7 @@ extern "C" int promp_env_observe_module(void* module, int n_env, const float* st
     PROMP_REQUIRE(n_env > 0 && state && obs, "%s: bad arguments", fn);
     void* args[] = {&n_env, &state, &obs};
     const int bs = 128;
-    return launch(fn, m, PROMP_ENV_SLOT_OBSERVE, dim3((n_env + bs - 1) / bs), dim3(bs), args, (cudaStream_t)stream);
+    return launch(fn, m, PROMP_ENV_SLOT_OBSERVE, dim3((n_env + bs - 1) / bs), dim3(bs), args, 0, (cudaStream_t)stream);
 }
 
 extern "C" int promp_cuda_build_version(void) { return CUDART_VERSION; }

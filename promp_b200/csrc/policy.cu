@@ -1239,6 +1239,10 @@ static int launch_forward(int M, int N, const float* params, int64_t stride, con
     return PROMP_OK;
 }
 
+}  // namespace promp
+#include "policy_deep.cuh"
+namespace promp {
+
 // the instantiation for this translation unit's activation; hid_ = the width decoded from `hidden`
 #define PROMP_DISPATCH_ACT(FN, DO, DA, HID, ...) return FN<DO, DA, HID, PROMP_POLICY_ACT>(__VA_ARGS__);
 
@@ -1300,6 +1304,21 @@ int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, con
             float* mean, cudaStream_t s) {
     PROMP_DISPATCH(launch_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, s)
 }
+// policies of depth 1 and 3 (policy_deep.cuh); nh = depth - 1
+int deep_grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_deep_grad, A, nh, ws, ws_bytes, s)
+}
+int deep_hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_deep_hvp, A, nh, ws, ws_bytes, s)
+}
+int deep_chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,
+               const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_deep_chain, n_stages, kinds, A, nh, skip_flag, skip_theta, ws, ws_bytes, s)
+}
+int deep_forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params, int64_t stride,
+                 const float* obs, float* mean, cudaStream_t s) {
+    PROMP_DISPATCH(launch_deep_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, nh, s)
+}
 }  // namespace PROMP_ACT_NS
 
 #ifndef PROMP_POLICY_EXTRA_TU
@@ -1315,6 +1334,14 @@ int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, con
               const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);                         \
     int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride,             \
                 const float* obs, float* mean, cudaStream_t s);                                                                   \
+    int deep_grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes,           \
+                  cudaStream_t s);                                                                                                \
+    int deep_hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes,            \
+                 cudaStream_t s);                                                                                                 \
+    int deep_chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,      \
+                   const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);                    \
+    int deep_forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params,                \
+                     int64_t stride, const float* obs, float* mean, cudaStream_t s);                                              \
     }
 PROMP_DECLARE_UNIT(relu_tu)
 PROMP_DECLARE_UNIT(otanh_tu)
@@ -1323,9 +1350,9 @@ PROMP_DECLARE_UNIT(relu_otanh_tu)
 
 // checks `hidden` (decode_hidden) and decodes its activations; returns from the caller on bad bits
 #define PROMP_DECODE_HIDDEN(who)                                                                 \
-    int hid_ = 0;                                                                                \
+    int hid_ = 0, depth_ = 2;                                                                    \
     bool relu_ = false, otanh_ = false;                                                          \
-    if (decode_hidden(who, hidden, hid_, relu_, otanh_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    if (decode_hidden(who, hidden, hid_, relu_, otanh_, depth_) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
 // dispatch function FN of the unit that holds the decoded activations' kernels
 #define PROMP_UNIT(FN) (otanh_ ? (relu_ ? relu_otanh_tu::FN : otanh_tu::FN) : (relu_ ? relu_tu::FN : tanh_tu::FN))
 
@@ -1351,9 +1378,9 @@ extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int a
 
 extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]) {
     PROMP_REQUIRE(out != nullptr, "promp_policy_layout: null output");
-    int width;           // the activations do not change the layout
+    int width, depth;    // the activations do not change the layout; the depth does
     bool relu, out_tanh;
-    if (decode_hidden("promp_policy_layout", hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    if (decode_hidden("promp_policy_layout", hidden, width, relu, out_tanh, depth) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     hidden = width;
     PROMP_REQUIRE(obs_dim >= 1 && obs_dim <= 19 && act_dim >= 1 && act_dim <= 8 && (hidden == 32 || hidden == 64),
                   "promp_policy_layout: padded policy kernels take obs_dim in [1, 19], act_dim in [1, 8] and hidden 32 or 64 "
@@ -1361,7 +1388,7 @@ extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t
     out[0] = obs_dim <= 8 ? 8 : 20;
     out[1] = act_dim <= 2 ? 2 : 8;
     out[2] = hidden;
-    out[3] = promp::num_params(out[0], out[1], hidden);
+    out[3] = promp::num_params(out[0], out[1], hidden, depth);
     return PROMP_OK;
 }
 
@@ -1412,6 +1439,7 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
     explore_args(A);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_grad")
+    if (depth_ != 2) return PROMP_UNIT(deep_grad)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
     return PROMP_UNIT(grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
@@ -1471,6 +1499,7 @@ static int policy_hvp_impl(bool padded, int obs_dim, int act_dim, int hidden, in
     A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_hvp")
+    if (depth_ != 2) return PROMP_UNIT(deep_hvp)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
     return PROMP_UNIT(hvp)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
 }
 
@@ -1566,6 +1595,13 @@ static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int a
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_workspace_bytes")
+    if (depth_ != 2) {      // one launch per stage: the control words, then the workspace of the largest stand-alone launch
+        int nmax = 1;
+        for (int k = 0; k < n_stages; ++k) nmax = Ns[k] > nmax ? Ns[k] : nmax;
+        const int64_t single = padded ? promp_policy_workspace_bytes_padded(M, nmax, obs_dim, act_dim, hidden)
+                                      : promp_policy_workspace_bytes(M, nmax, obs_dim, act_dim, hidden);
+        return single < 0 ? -1 : chain_ctrl_bytes(M) + single;
+    }
     return PROMP_UNIT(chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
 }
 extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
@@ -1583,6 +1619,7 @@ static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim,
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_num_launches")
+    if (depth_ != 2) return n_stages;
     return PROMP_UNIT(chain_launches)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
 }
 extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
@@ -1632,6 +1669,9 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
     }
     const int rc_clear = chain_clear_on_new_m(workspace, M, s);
     if (rc_clear != PROMP_OK) return rc_clear;
+    if (depth_ != 2)
+        return PROMP_UNIT(deep_chain)(padded, obs_dim, act_dim, hidden, depth_ - 1, n_stages, kinds, A, skip_flag, skip_theta,
+                                      workspace, workspace_bytes, s);
     return PROMP_UNIT(chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta, workspace,
                              workspace_bytes, s);
 }
@@ -1682,6 +1722,7 @@ static int policy_forward_impl(bool padded, int obs_dim, int act_dim, int hidden
     PROMP_REQUIRE(M <= 65535, "promp_policy_forward: M=%d exceeds the grid.y limit", M);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_forward")
+    if (depth_ != 2) return PROMP_UNIT(deep_forward)(padded, obs_dim, act_dim, hidden, depth_ - 1, M, N, params, param_stride, obs, mean, s);
     return PROMP_UNIT(forward)(padded, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, s);
 }
 extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,

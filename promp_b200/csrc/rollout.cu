@@ -28,12 +28,49 @@ static int with_env(const char* fn, int env_kind, F&& f) {
     return PROMP_ERR_INVALID_ARG;
 }
 
-// `hidden` as decode_hidden gives it: width 32 or 64, ReLU or tanh, identity or tanh output
-static int launch_rollout(const char* fn, int env_kind, int width, bool relu, bool out_tanh, const RolloutArgs& A,
+// rollout_deep_kernel for a policy of depth 1 or 3: its hidden-to-hidden layers take dynamic shared memory beyond the
+// 48 KB default, so the limit is raised once per instantiation
+template <class Env, int HID, class Act, bool K>
+static int launch_rollout_deep(const RolloutArgs& A, int nh, dim3 grid, cudaStream_t st) {
+    static bool configured = false;
+    constexpr auto kernel = rollout_deep_kernel<Env, HID, Act, K>;
+    if (!configured) {
+        PROMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, rollout_deep_smem_bytes<HID>(2)));
+        configured = true;
+    }
+    kernel<<<grid, RO_WARPS * 32, rollout_deep_smem_bytes<HID>(nh), st>>>(A, nh);
+    return PROMP_OK;
+}
+
+template <class Env, bool K>
+static int launch_rollout_deep_act(int width, bool relu, bool out_tanh, const RolloutArgs& A, int nh, dim3 grid,
+                                   cudaStream_t st) {
+    using OR = OutTanh<ActRelu>;
+    using OT = OutTanh<ActTanh>;
+    if (out_tanh) {
+        if (relu) return width == 64 ? launch_rollout_deep<Env, 64, OR, K>(A, nh, grid, st) : launch_rollout_deep<Env, 32, OR, K>(A, nh, grid, st);
+        return width == 64 ? launch_rollout_deep<Env, 64, OT, K>(A, nh, grid, st) : launch_rollout_deep<Env, 32, OT, K>(A, nh, grid, st);
+    }
+    if (relu)
+        return width == 64 ? launch_rollout_deep<Env, 64, ActRelu, K>(A, nh, grid, st)
+                           : launch_rollout_deep<Env, 32, ActRelu, K>(A, nh, grid, st);
+    return width == 64 ? launch_rollout_deep<Env, 64, ActTanh, K>(A, nh, grid, st)
+                       : launch_rollout_deep<Env, 32, ActTanh, K>(A, nh, grid, st);
+}
+
+// `hidden` as decode_hidden gives it: width 32 or 64, ReLU or tanh, identity or tanh output, 1 to 3 hidden layers
+static int launch_rollout(const char* fn, int env_kind, int width, bool relu, bool out_tanh, int depth, const RolloutArgs& A,
                           cudaStream_t st) {
     const dim3 grid((A.E + RO_WARPS - 1) / RO_WARPS, A.M);
     return with_env(fn, env_kind, [&](auto env) -> int {
         using Env = typename decltype(env)::type;
+        if (depth != 2) {
+            const int rc = A.key_offset ? launch_rollout_deep_act<Env, true>(width, relu, out_tanh, A, depth - 1, grid, st)
+                                        : launch_rollout_deep_act<Env, false>(width, relu, out_tanh, A, depth - 1, grid, st);
+            if (rc != PROMP_OK) return rc;
+            PROMP_LAUNCH_CHECK("rollout_deep_kernel");
+            return PROMP_OK;
+        }
         const auto go = [&](auto keyed) {
             constexpr bool K = decltype(keyed)::value;
             if (out_tanh) {
@@ -82,9 +119,9 @@ static int rollout_fixed(const char* fn, int env_kind, int reward_type, float sp
     PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
     if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
-    int width;
+    int width, depth;
     bool relu, out_tanh;
-    if (decode_hidden(fn, hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    if (decode_hidden(fn, hidden, width, relu, out_tanh, depth) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
     PROMP_REQUIRE(reward_type >= 0 && reward_type <= 2, "%s: bad reward_type %d", fn, reward_type);
     PROMP_REQUIRE(env_kind != PROMP_ENV_CHEETAH_DIR || info != nullptr,
@@ -100,7 +137,7 @@ static int rollout_fixed(const char* fn, int env_kind, int reward_type, float sp
     RolloutArgs A{reward_type, sparse_radius, normalize_actions, M, E, H, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, info, log_std_out,
                   final_state, 0, H, (uint32_t)task_offset * (uint32_t)E};
-    return launch_rollout(fn, env_kind, width, relu, out_tanh, A, (cudaStream_t)stream);
+    return launch_rollout(fn, env_kind, width, relu, out_tanh, depth, A, (cudaStream_t)stream);
 }
 
 extern "C" int promp_rollout(int env_kind, int reward_type, float sparse_radius, int normalize_actions, int M, int E, int H,
@@ -140,14 +177,14 @@ static int rollout_early_term(const char* fn, int env_kind, int normalize_action
     PROMP_REQUIRE(M <= 65535, "%s: M=%d exceeds the grid.y limit 65535", fn, M);
     if (check_task_offset(fn, task_offset, M, E) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(params && task_params && obs && act && mean && rew && done && log_std_out, "%s: null pointer argument", fn);
-    int width;
+    int width, depth;
     bool relu, out_tanh;
-    if (decode_hidden(fn, hidden, width, relu, out_tanh) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
+    if (decode_hidden(fn, hidden, width, relu, out_tanh, depth) != PROMP_OK) return PROMP_ERR_INVALID_ARG;
     PROMP_REQUIRE(width == 64 || width == 32, "%s: hidden size %d unsupported (32 or 64)", fn, width);
     RolloutArgs A{0, 0.f, normalize_actions, M, E, timeline_len, params, param_stride, task_params, init_state, noise, seed,
                   stream_id, stream_id_dev, clip_reported_log_std, min_log_std, obs, act, mean, rew, done, nullptr, log_std_out,
                   nullptr, 1, horizon, (uint32_t)task_offset * (uint32_t)E};
-    return launch_rollout(fn, env_kind, width, relu, out_tanh, A, (cudaStream_t)stream);
+    return launch_rollout(fn, env_kind, width, relu, out_tanh, depth, A, (cudaStream_t)stream);
 }
 
 extern "C" int promp_rollout_early_term(int env_kind, int normalize_actions, int M, int E, int timeline_len, int horizon, int hidden,

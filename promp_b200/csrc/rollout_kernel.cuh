@@ -312,6 +312,211 @@ __global__ void __launch_bounds__(RO_WARPS * 32) rollout_kernel(RolloutArgs A) {
     if (A.final_state) env.store(A.final_state + env_id * SD, lane);
 }
 
+// ---------------------------------------------------------------------------- policies of depth 1 and 3
+// rollout_kernel for a policy with nh = depth - 1 hidden-to-hidden layers (0 or 2, a kernel argument: one instantiation
+// serves both depths).  A 64 x 64 matrix does not fit the registers of a warp next to the env (it alone is 128 registers per
+// lane), so the hidden-to-hidden layers [W_1 b_1 W_2 b_2] live in dynamic shared memory, staged once per CTA: the RO_WARPS
+// warps of a CTA step envs of the same task and share that copy.  Layer 0, the output layer and the env step are those of
+// rollout_kernel; lane j reads row k of a hidden matrix at k * HID + j (conflict-free) and the activation as a broadcast.
+template <int HID>
+__host__ __device__ constexpr int rollout_deep_smem_bytes(int nh) {
+    return nh * (HID * HID + HID) * (int)sizeof(float);
+}
+
+template <class Env, int HID, class Act, bool KEYED>
+__global__ void __launch_bounds__(RO_WARPS * 32) rollout_deep_kernel(RolloutArgs A, int nh) {
+    constexpr int DO = Env::DO, DA = Env::DA, SD = Env::SD, TD = Env::TD;
+    constexpr int NU = HID / 32;
+    constexpr int DAP = PolicyCaps<DO, DA>::ACT;
+    const DeepLayout<PolicyCaps<DO, DA>::OBS, DAP, HID> L{nh};
+    static_assert(HID % 32 == 0, "hidden size must be a multiple of 32");
+
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int m = blockIdx.y, e = blockIdx.x * RO_WARPS + w;
+
+    __shared__ __align__(16) RolloutSmem<Env, HID> smem_all[RO_WARPS];
+    extern __shared__ __align__(16) float s_wh[];       // [nh][HID * HID + HID]: W_l then b_l, as in the parameter vector
+    RolloutSmem<Env, HID>& S = smem_all[w];
+
+    const float* th = A.params + (int64_t)m * A.param_stride;
+    for (int i = threadIdx.x; i < nh * (HID * HID + HID); i += blockDim.x) s_wh[i] = __ldg(th + L.wh(0) + i);
+    __syncthreads();
+    if (e >= A.E) return;   // whole warp leaves; nothing below uses a block-wide barrier
+
+    if (A.stream_id_dev) A.stream_id += *A.stream_id_dev;
+    const int64_t env_id = (int64_t)m * A.E + e;
+    const int64_t base = env_id * A.H;
+
+    float w0[DO][NU], b0[NU], w2[NU][DA], b2[DA], sig[DA];
+#pragma unroll
+    for (int u = 0; u < NU; ++u) {
+        const int j = lane + 32 * u;
+#pragma unroll
+        for (int i = 0; i < DO; ++i) w0[i][u] = __ldg(th + L.W0 + i * HID + j);
+        b0[u] = __ldg(th + L.B0 + j);
+#pragma unroll
+        for (int d = 0; d < DA; ++d) w2[u][d] = __ldg(th + L.wo() + j * DAP + d);
+    }
+#pragma unroll
+    for (int d = 0; d < DA; ++d) {
+        b2[d] = __ldg(th + L.bo() + d);
+        float ls = __ldg(th + L.ls() + d);
+        sig[d] = expf(ls);
+        if (e == 0 && lane == d)
+            A.log_std_out[(int64_t)m * DA + d] = A.clip_reported ? fmaxf(ls, A.min_log_std) : ls;
+    }
+
+    float task[TD];
+#pragma unroll
+    for (int i = 0; i < TD; ++i) task[i] = __ldg(A.task_params + (int64_t)m * TD + i);
+
+    const EnvRng rng{KEYED ? (uint32_t)env_id + A.key_offset : (uint32_t)env_id, (uint32_t)A.stream_id,
+                     (uint32_t)((A.stream_id >> 32) & 0xffffffu), A.seed};
+    Env env;
+    if (A.init_state) env.load(A.init_state + env_id * SD, lane);
+    else env.reset(rng, 0u, 0x52000000u, lane, task);
+    env.observe(S.obs, lane);
+    __syncwarp();
+
+    const EnvCfg cfg{A.reward_type, A.radius, A.normalized != 0};
+    [[maybe_unused]] int path_ts = 0;
+
+    for (int t0 = 0; t0 < A.H; t0 += T_CH) {
+        const int nt = min(T_CH, A.H - t0);
+        if (A.noise) {
+            const float* ng = A.noise + (base + t0) * DA;
+            for (int i = lane; i < nt * DA; i += 32) S.noise[i] = __ldg(ng + i);
+        } else if (lane < nt) {
+            const int t = t0 + lane;
+#pragma unroll
+            for (int blk = 0; blk < (DA + 3) / 4; ++blk) {
+                uint32_t r[4];
+                rng.gen((uint32_t)t, (uint32_t)blk << 24, r);
+                float z[4];
+                box_muller(r[0], r[1], z[0], z[1]);
+                box_muller(r[2], r[3], z[2], z[3]);
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                    if (blk * 4 + i < DA) S.noise[lane * DA + blk * 4 + i] = z[i];
+            }
+        }
+        __syncwarp();
+
+        for (int tt = 0; tt < nt; ++tt) {
+            // ---- layer 0: h = act(obs W0 + b0)            (policies/networks/mlp.py:96-117)
+            float ob[DO], h[NU];
+#pragma unroll
+            for (int i = 0; i < DO; ++i) ob[i] = S.obs[i];
+#pragma unroll
+            for (int u = 0; u < NU; ++u) {
+                float z = b0[u];
+#pragma unroll
+                for (int i = 0; i < DO; ++i) z = fmaf(ob[i], w0[i][u], z);
+                h[u] = Act::f(z);
+                S.h1[lane + 32 * u] = h[u];
+            }
+            if (lane < DO) S.st_obs[tt * DO + lane] = S.obs[lane];
+            __syncwarp();
+            // ---- hidden layers: h = act(h W_l + b_l), weights from shared memory
+            for (int l = 0; l < nh; ++l) {
+                const float* Wl = s_wh + l * (HID * HID + HID);
+                float acc[NU][4];
+#pragma unroll
+                for (int u = 0; u < NU; ++u) {
+                    acc[u][0] = Wl[HID * HID + lane + 32 * u];
+                    acc[u][1] = acc[u][2] = acc[u][3] = 0.f;
+                }
+#pragma unroll 4
+                for (int k4 = 0; k4 < HID / 4; ++k4) {
+                    const float4 hv = *reinterpret_cast<const float4*>(&S.h1[4 * k4]);
+#pragma unroll
+                    for (int u = 0; u < NU; ++u) {
+                        const int j = lane + 32 * u;
+                        acc[u][0] = fmaf(hv.x, Wl[(4 * k4 + 0) * HID + j], acc[u][0]);
+                        acc[u][1] = fmaf(hv.y, Wl[(4 * k4 + 1) * HID + j], acc[u][1]);
+                        acc[u][2] = fmaf(hv.z, Wl[(4 * k4 + 2) * HID + j], acc[u][2]);
+                        acc[u][3] = fmaf(hv.w, Wl[(4 * k4 + 3) * HID + j], acc[u][3]);
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < NU; ++u) h[u] = Act::f((acc[u][0] + acc[u][1]) + (acc[u][2] + acc[u][3]));
+                __syncwarp();      // every lane has read this layer's input
+#pragma unroll
+                for (int u = 0; u < NU; ++u) S.h1[lane + 32 * u] = h[u];
+                __syncwarp();
+            }
+            // ---- output layer: mean = h W_out + b_out (warp shuffle reduction over the hidden units)
+            float mu[DA];
+#pragma unroll
+            for (int d = 0; d < DA; ++d) mu[d] = 0.f;
+#pragma unroll
+            for (int u = 0; u < NU; ++u)
+#pragma unroll
+                for (int d = 0; d < DA; ++d) mu[d] = fmaf(h[u], w2[u][d], mu[d]);
+#pragma unroll
+            for (int d = 0; d < DA; ++d) mu[d] = warp_sum(mu[d]) + b2[d];
+            out_forward<Act, DA>(mu);
+
+            float a[DA];
+#pragma unroll
+            for (int d = 0; d < DA; ++d) a[d] = fmaf(S.noise[tt * DA + d], sig[d], mu[d]);
+            if (lane < DA) {
+                float al = 0.f, ml = 0.f;
+#pragma unroll
+                for (int d = 0; d < DA; ++d)
+                    if (lane == d) al = a[d], ml = mu[d];
+                S.st_act[tt * DA + lane] = al;
+                S.st_mean[tt * DA + lane] = ml;
+            }
+
+            bool dn = false;
+            const float r = env.step(a, task, cfg, lane, S.st_info + tt, T_CH, dn);
+            if constexpr (Env::ENDS_EARLY) {
+                if (A.early_term) {
+                    ++path_ts;
+                    const bool fin = dn || path_ts >= A.horizon;
+                    if (lane == 0) S.st_done[tt] = fin ? 1 : 0;
+                    if (fin) {
+                        env.reset(rng, (uint32_t)(t0 + tt), 0x53000000u, lane, task);
+                        path_ts = 0;
+                    }
+                }
+            }
+            if (lane == 0) S.st_rew[tt] = r;
+            __syncwarp();
+            env.observe(S.obs, lane);
+            __syncwarp();
+        }
+
+        {
+            float* g;
+            g = A.obs + (base + t0) * DO;
+            for (int i = lane; i < nt * DO; i += 32) g[i] = S.st_obs[i];
+            g = A.act + (base + t0) * DA;
+            for (int i = lane; i < nt * DA; i += 32) g[i] = S.st_act[i];
+            g = A.mean + (base + t0) * DA;
+            for (int i = lane; i < nt * DA; i += 32) g[i] = S.st_mean[i];
+            if (lane < nt) {
+                A.rew[base + t0 + lane] = S.st_rew[lane];
+                A.done[base + t0 + lane] = A.early_term ? S.st_done[lane] : ((t0 + lane == A.H - 1) ? 1 : 0);
+                if (Env::NINFO > 0 && A.info) {
+                    const int64_t tot = (int64_t)A.M * A.E * A.H;
+                    if constexpr (generic_info<Env>::value) {
+#pragma unroll
+                        for (int c = 0; c < Env::NINFO; ++c) A.info[c * tot + base + t0 + lane] = S.st_info[c * T_CH + lane];
+                    } else {
+                        A.info[base + t0 + lane] = S.st_info[lane];
+                        A.info[tot + base + t0 + lane] = S.st_info[T_CH + lane];
+                        if (A.reward_type == 1) A.info[2 * tot + base + t0 + lane] = S.st_info[2 * T_CH + lane];
+                    }
+                }
+            }
+        }
+        __syncwarp();
+    }
+    if (A.final_state) env.store(A.final_state + env_id * SD, lane);
+}
+
 // ---------------------------------------------------------------------------- single-step kernels
 template <class Env>
 __global__ void env_step_kernel(EnvCfg cfg, int n_env, int H, float* state, int32_t* ts, const float* actions,

@@ -19,6 +19,16 @@ PARAM_NAMES = ('mean_network/hidden_0/kernel', 'mean_network/hidden_0/bias',
                'mean_network/hidden_1/kernel', 'mean_network/hidden_1/bias',
                'mean_network/output/kernel', 'mean_network/output/bias',
                'log_std_network/log_std_var')
+MAX_DEPTH = 3          # hidden layers: 1 to 3 (two run the kernels of PARAM_NAMES above, one and three kernels of their own)
+
+
+def param_names(depth):
+    """Variable names of a policy with `depth` hidden layers, in the reference's creation order (policies/networks/mlp.py:5-62:
+    hidden_0 .. hidden_{depth-1}, output; gaussian_mlp_policy.py:55-80: log_std)."""
+    names = []
+    for i in range(depth):
+        names += ['mean_network/hidden_%d/kernel' % i, 'mean_network/hidden_%d/bias' % i]
+    return tuple(names) + PARAM_NAMES[4:]
 # (obs_dim, action_dim) with policy kernels of their own; every other shape in range runs on the zero-padded kernels
 EXACT_SHAPES = ((2, 2), (4, 2), (17, 6))
 MAX_OBS_DIM, MAX_ACTION_DIM = 19, 8
@@ -49,9 +59,9 @@ class MetaGaussianMLPPolicy(object):
         import torch
         _lib.require_cuda()
         hidden_sizes = tuple(int(h) for h in hidden_sizes)
-        if len(hidden_sizes) != 2 or max(hidden_sizes) > 64 or min(hidden_sizes) < 1:
-            raise NotImplementedError("promp_b200 kernels are built for two tanh hidden layers of up to 64 units each "
-                                      "(got hidden_sizes=%r)" % (hidden_sizes,))
+        if not 1 <= len(hidden_sizes) <= MAX_DEPTH or max(hidden_sizes) > 64 or min(hidden_sizes) < 1:
+            raise NotImplementedError("promp_b200 kernels are built for 1 to %d hidden layers of up to 64 units each "
+                                      "(got hidden_sizes=%r)" % (MAX_DEPTH, hidden_sizes))
         if not (1 <= int(obs_dim) <= MAX_OBS_DIM and 1 <= int(action_dim) <= MAX_ACTION_DIM):
             raise NotImplementedError("promp_b200 policy kernels take obs_dim in [1, %d] and action_dim in [1, %d] (got %d, %d)"
                                       % (MAX_OBS_DIM, MAX_ACTION_DIM, int(obs_dim), int(action_dim)))
@@ -77,27 +87,33 @@ class MetaGaussianMLPPolicy(object):
         self.output_nonlinearity = out        # None (identity) or 'tanh'
         # the `hidden` argument of every policy / rollout kernel call: the width, plus the activation flag for ReLU and the
         # output flag for a tanh mean
-        self.hidden_arg = self.hidden | (_lib.ACT_RELU if act == 'relu' else 0) | (_lib.OUT_TANH if out == 'tanh' else 0)
+        # output flag for a tanh mean, and the depth bits for one or three hidden layers (none for two)
+        self.depth = len(hidden_sizes)
+        self.hidden_arg = (self.hidden | (_lib.ACT_RELU if act == 'relu' else 0) | (_lib.OUT_TANH if out == 'tanh' else 0)
+                           | _lib.hidden_depth(self.depth))
         self.learn_std = learn_std
         self.min_log_std = math.log(min_std)
         self.init_log_std = math.log(init_std)
         self.device = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
         self._dist = DiagonalGaussian(self.action_dim)
-        h0, h1, Hd = hidden_sizes[0], hidden_sizes[1], self.hidden
-        self.param_shapes = OrderedDict(zip(PARAM_NAMES, (
-            (self.obs_dim, h0), (h0,), (h0, h1), (h1,), (h1, self.action_dim), (self.action_dim,), (1, self.action_dim))))
+        Hd, names = self.hidden, param_names(self.depth)
+        ins = (self.obs_dim,) + hidden_sizes
+        shapes = [s for i in range(self.depth) for s in ((ins[i], ins[i + 1]), (ins[i + 1],))]
+        self.param_shapes = OrderedDict(zip(names, shapes + [(hidden_sizes[-1], self.action_dim), (self.action_dim,),
+                                                             (1, self.action_dim)]))
         self.num_params_logical = int(sum(np.prod(sh) for sh in self.param_shapes.values()))
         # Shapes outside EXACT_SHAPES pad the observation and action axes the same way: W0 gets zero rows up to obs_cap,
         # W2 / b2 / log_std zero columns up to act_cap (promp_policy_layout), and the padded kernels keep them at zero.
         self.padded_dims = (self.obs_dim, self.action_dim) not in EXACT_SHAPES
         if self.padded_dims:
-            do_cap, da_cap, _, _ = _lib.policy_layout(self.obs_dim, self.action_dim, Hd)
+            do_cap, da_cap, _, _ = _lib.policy_layout(self.obs_dim, self.action_dim, self.hidden_arg)
         else:
             do_cap, da_cap = self.obs_dim, self.action_dim
         self.entries = {k: 'promp_policy_' + k + ('_padded' if self.padded_dims else '') for k in POLICY_ENTRIES}
-        dev_shapes = ((do_cap, Hd), (Hd,), (Hd, Hd), (Hd,), (Hd, da_cap), (da_cap,), (1, da_cap))
+        dev_shapes = (((do_cap, Hd), (Hd,)) + ((Hd, Hd), (Hd,)) * (self.depth - 1)
+                      + ((Hd, da_cap), (da_cap,), (1, da_cap)))
         self.num_params = int(sum(np.prod(sh) for sh in dev_shapes))          # device (padded) vector length
-        assert self.num_params == _lib.load().promp_num_params(do_cap, da_cap, self.hidden)
+        assert self.num_params == _lib.load().promp_num_params(do_cap, da_cap, self.hidden_arg)
         # positions of the logical parameters inside the padded device vector
         idx, off = [], 0
         for (key, shape), dshape in zip(self.param_shapes.items(), dev_shapes):
@@ -106,7 +122,7 @@ class MetaGaussianMLPPolicy(object):
             off += int(np.prod(dshape))
         self._pad_index_np = np.concatenate(idx)
         self._log_std_lo = self.num_params - da_cap        # the logical log_std: [lo, lo + action_dim) of the device vector
-        self.policy_params_keys = list(PARAM_NAMES)
+        self.policy_params_keys = list(names)
         # Xavier-uniform kernels, zero biases, log_std = log(init_std)
         # (policies/networks/mlp.py:12-13, gaussian_mlp_policy.py:64-69); drawn from the numpy global RNG
         flat = []
