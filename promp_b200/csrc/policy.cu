@@ -760,6 +760,10 @@ __global__ void __launch_bounds__(128) policy_forward_otanh_kernel(int M, int N,
     policy_forward_body<DO, DA, HID, OutTanh<Hid>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
 }
 
+}  // namespace promp
+#include "policy_deep.cuh"
+namespace promp {
+
 #ifndef PROMP_POLICY_EXTRA_TU
 __global__ void reduce_tasks_kernel(int M, int P, const float* in, float scale, float* out) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -951,10 +955,24 @@ static int sm_count() {
     return n;
 }
 static int64_t counters_bytes(int M) { return (((int64_t)M * sizeof(int) + 15) / 16) * 16; }
+// Workspace of one launch over a P-parameter policy: an upper bound over the occupancies the kernels can have (1..4 CTAs per
+// SM on this device's SMs, or on 160)
+static int64_t policy_workspace_bytes(int M, int N, int P) {
+    int64_t worst = 0;
+    for (int occ = 1; occ <= 4; ++occ)
+        for (int tb : {TB, TBT}) {            // CUDA-core kernels tile by 64 samples, the tensor-core kernels by 128
+            const TilePlan p = plan_tiles(M, N, 160 * occ, P, tb);
+            if (p.partial_floats > worst) worst = p.partial_floats;
+            const TilePlan p2 = plan_tiles(M, N, sm_count() * occ, P, tb);
+            if (p2.partial_floats > worst) worst = p2.partial_floats;
+        }
+    return counters_bytes(M) + worst * (int64_t)sizeof(float) + 16;
+}
 
-template <typename Kernel>
+// One persistent launch over tb-sample tiles; `extra`: the kernel's arguments after A (nh for the kernels of policy_deep.cuh)
+template <typename Kernel, typename... Extra>
 static int launch_policy(Kernel kernel, int smem, int& occ_cache, PolicyArgs& A, int P, void* ws, int64_t ws_bytes,
-                         cudaStream_t st, const char* name, int tb = TB, int threads = PT_THREADS) {
+                         cudaStream_t st, const char* name, int tb, int threads, Extra... extra) {
     if (occ_cache == 0) {
         PROMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         int occ = 0;
@@ -971,7 +989,7 @@ static int launch_policy(Kernel kernel, int smem, int& occ_cache, PolicyArgs& A,
     A.partial = (float*)((char*)ws + counters_bytes(A.M));
     A.q = p.q;
     A.kmax = p.kmax;
-    kernel<<<p.grid, threads, smem, st>>>(A);
+    kernel<<<p.grid, threads, smem, st>>>(A, extra...);
     PROMP_LAUNCH_CHECK(name);
     return PROMP_OK;
 }
@@ -988,24 +1006,38 @@ constexpr bool is_relu() { return std::is_same<Act, ActRelu>::value; }
         else return NAME##_kernel<__VA_ARGS__>;                                                        \
     }()
 
+// nh = the number of hidden-to-hidden layers (depth - 1).  Two hidden layers run the tensor-core kernels (hidden 64) or the
+// two-layer CUDA-core kernels above; one and three run the depth-generic CUDA-core kernels of policy_deep.cuh.
 template <int DO, int DA, int HID, class Act>
-static int launch_grad(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
+static int launch_grad(PolicyArgs& A, int nh, void* ws, int64_t ws_bytes, cudaStream_t st) {
+    if (nh != 1) {
+        const int P = DeepLayout<DO, DA, HID>{nh}.P();
+        constexpr int smem = (int)sizeof(DeepGradSmem<DO, DA, HID>);
+        if (A.adv_per_task) {
+            static int occ_x = 0;
+            return launch_policy(policy_grad_deep_kernel<DO, DA, HID, Act, ADV_TASK>, smem, occ_x, A, P, ws, ws_bytes, st,
+                                 "policy_grad_deep_kernel", TB, PT_THREADS, nh);
+        }
+        static int occ = 0;
+        return launch_policy(policy_grad_deep_kernel<DO, DA, HID, Act, ADV_SAMPLE>, smem, occ, A, P, ws, ws_bytes, st,
+                             "policy_grad_deep_kernel", TB, PT_THREADS, nh);
+    }
     if (A.adv_per_task) {
         static int occ_x = 0;
         constexpr auto kx = PROMP_ACT_KERNEL(Act, policy_grad_explore, DO, DA, HID);
         return launch_policy(kx, (int)sizeof(GradSmem<DO, DA, HID>), occ_x, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
-                             "policy_grad_explore_kernel");
+                             "policy_grad_explore_kernel", TB, PT_THREADS);
     }
     static int occ = 0;
     constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_grad, DO, DA, HID);
     return launch_policy(kernel, (int)sizeof(GradSmem<DO, DA, HID>), occ, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
-                         "policy_grad_kernel");
+                         "policy_grad_kernel", TB, PT_THREADS);
 }
 
 template <int DO, int DA, int HID, class Act>
-static int launch_grad_any(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
+static int launch_grad_any(PolicyArgs& A, int nh, void* ws, int64_t ws_bytes, cudaStream_t st) {
     if constexpr (HID == TC_HID) {
-        if (g_use_tc && A.adv_per_task) {
+        if (g_use_tc && nh == 1 && A.adv_per_task) {
             static int occ2 = 0, occ4 = 0;
             constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_grad_tc_explore, DO, DA, 4);
             constexpr auto k2 = PROMP_ACT_KERNEL(Act, policy_grad_tc_explore, DO, DA, 2);
@@ -1015,7 +1047,7 @@ static int launch_grad_any(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream
             return launch_policy(k2, (int)sizeof(GradTcSmem<DO, DA, 2>), occ2, A,
                                  PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_explore_kernel", TBT, 256);
         }
-        if (g_use_tc) {
+        if (g_use_tc && nh == 1) {
             static int occ2 = 0, occ4 = 0;
             constexpr auto k4 = PROMP_ACT_KERNEL(Act, policy_grad_tc, DO, DA, 4);
             constexpr auto k2 = PROMP_ACT_KERNEL(Act, policy_grad_tc, DO, DA, 2);
@@ -1026,11 +1058,17 @@ static int launch_grad_any(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream
                                  PLayout<DO, DA, HID>::P, ws, ws_bytes, st, "policy_grad_tc_kernel", TBT, 256);
         }
     }
-    return launch_grad<DO, DA, HID, Act>(A, ws, ws_bytes, st);
+    return launch_grad<DO, DA, HID, Act>(A, nh, ws, ws_bytes, st);
 }
 
 template <int DO, int DA, int HID, class Act>
-static int launch_hvp(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st) {
+static int launch_hvp(PolicyArgs& A, int nh, void* ws, int64_t ws_bytes, cudaStream_t st) {
+    if (nh != 1) {
+        static_assert(sizeof(DeepHvpSmem<DO, DA, HID>) <= 227 * 1024, "deep HVP tile exceeds the shared memory of one SM");
+        static int occ = 0;
+        return launch_policy(policy_hvp_deep_kernel<DO, DA, HID, Act>, (int)sizeof(DeepHvpSmem<DO, DA, HID>), occ, A,
+                             DeepLayout<DO, DA, HID>{nh}.P(), ws, ws_bytes, st, "policy_hvp_deep_kernel", TB, PT_THREADS, nh);
+    }
     if constexpr (HID == TC_HID && sizeof(HvpTcSmem<DO, DA, 2>) <= 227 * 1024) {     // fits the 227 KB of one SM
         if (g_use_tc) {
             static int occ2 = 0, occ4 = 0;
@@ -1046,7 +1084,7 @@ static int launch_hvp(PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t st
     static int occ = 0;
     constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_hvp, DO, DA, HID);
     return launch_policy(kernel, (int)sizeof(HvpSmem<DO, DA, HID>), occ, A, PLayout<DO, DA, HID>::P, ws, ws_bytes, st,
-                         "policy_hvp_kernel");
+                         "policy_hvp_kernel", TB, PT_THREADS);
 }
 
 // ---- dataflow chain (policy_chain_tc_kernel): work-item plan + launch ---------------------------------------------
@@ -1154,17 +1192,17 @@ static int launch_chain_nq(ChainArgs& C, cudaStream_t st) {
 }
 
 // kinds / Ns / A: the stages in order.  Falls back to one launch per stage (same results up to summation order) for the
-// shapes the tensor-core kernels do not cover or when the "chain" option is off.
+// shapes and depths the tensor-core kernels do not cover (the dataflow kernel is built for two hidden layers) or when the
+// "chain" option is off.
 template <int DO, int DA, int HID, class Act>
-static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag, const float* skip_theta, void* ws,
-                        int64_t ws_bytes, cudaStream_t st) {
-    constexpr int P = PLayout<DO, DA, HID>::P;
+static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, int nh, const int* skip_flag, const float* skip_theta,
+                        void* ws, int64_t ws_bytes, cudaStream_t st) {
     int Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) Ns[s] = A[s].N;
     const int M = A[0].M;
-    const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, P);
+    const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, DeepLayout<DO, DA, HID>{nh}.P());
     if constexpr (chain_tc_ok<DO, DA, HID>()) {
-        if (chain_uses_dataflow(pl, n_stages, M)) {
+        if (nh == 1 && chain_uses_dataflow(pl, n_stages, M)) {
             if (ws_bytes < pl.bytes) {
                 set_error("policy chain workspace too small (%lld < %lld bytes)", (long long)ws_bytes, (long long)pl.bytes);
                 return PROMP_ERR_WORKSPACE;
@@ -1200,8 +1238,8 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
     for (int s = 0; s < n_stages; ++s) {
         PolicyArgs a = A[s];
         if (s == 0) a.skip_flag = skip_flag, a.skip_theta = skip_theta;
-        const int rc = kinds[s] == 0 ? launch_grad_any<DO, DA, HID, Act>(a, ws1, ws1_bytes, st)
-                                     : launch_hvp<DO, DA, HID, Act>(a, ws1, ws1_bytes, st);
+        const int rc = kinds[s] == 0 ? launch_grad_any<DO, DA, HID, Act>(a, nh, ws1, ws1_bytes, st)
+                                     : launch_hvp<DO, DA, HID, Act>(a, nh, ws1, ws1_bytes, st);
         if (rc != PROMP_OK) return rc;
     }
     return PROMP_OK;
@@ -1209,39 +1247,44 @@ static int launch_chain(int n_stages, const int* kinds, PolicyArgs* A, const int
 
 // the activation does not change the plan: `Act` only keeps the dispatch uniform
 template <int DO, int DA, int HID, class Act>
-static int chain_num_launches(int n_stages, const int* kinds, const int* Ns, int M) {
+static int chain_num_launches(int n_stages, const int* kinds, const int* Ns, int M, int nh) {
     if constexpr (chain_tc_ok<DO, DA, HID>()) {
-        const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, PLayout<DO, DA, HID>::P);
-        if (chain_uses_dataflow(pl, n_stages, M)) return 1;
+        const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, DeepLayout<DO, DA, HID>{nh}.P());
+        if (nh == 1 && chain_uses_dataflow(pl, n_stages, M)) return 1;
     }
     return n_stages;
 }
 
+// The control words, then the workspace of the largest stand-alone launch; two hidden layers also reserve the dataflow
+// kernel's partial slots
 template <int DO, int DA, int HID, class Act>
-static int64_t chain_ws_bytes(int n_stages, const int* kinds, const int* Ns, int M) {
-    const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, PLayout<DO, DA, HID>::P);
+static int64_t chain_ws_bytes(int n_stages, const int* kinds, const int* Ns, int M, int nh) {
+    const int P = DeepLayout<DO, DA, HID>{nh}.P();
+    const ChainPlan pl = plan_chain(n_stages, kinds, Ns, M, P);
     int nmax = 1;
     for (int s = 0; s < n_stages; ++s) nmax = Ns[s] > nmax ? Ns[s] : nmax;
-    const int64_t single = pl.ctrl_bytes + promp_policy_workspace_bytes(M, nmax, DO, DA, HID);
-    return pl.bytes > single ? pl.bytes : single;
+    const int64_t single = pl.ctrl_bytes + policy_workspace_bytes(M, nmax, P);
+    return nh == 1 && pl.bytes > single ? pl.bytes : single;
 }
 
 template <int DO, int DA, int HID, class Act>
 static int launch_forward(int M, int N, const float* params, int64_t stride, const float* obs, float* mean, int obs_dim,
-                          int act_dim, cudaStream_t st) {
+                          int act_dim, int nh, cudaStream_t st) {
     int gx = (N + 3) / 4;
     const int cap = (4 * sm_count() + M - 1) / M;
     if (gx > cap) gx = cap;
     if (gx < 1) gx = 1;
+    if (nh != 1) {
+        policy_forward_deep_kernel<DO, DA, HID, Act><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim,
+                                                                                   act_dim, nh);
+        PROMP_LAUNCH_CHECK("policy_forward_deep_kernel");
+        return PROMP_OK;
+    }
     constexpr auto kernel = PROMP_ACT_KERNEL(Act, policy_forward, DO, DA, HID);
     kernel<<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim);
     PROMP_LAUNCH_CHECK("policy_forward_kernel");
     return PROMP_OK;
 }
-
-}  // namespace promp
-#include "policy_deep.cuh"
-namespace promp {
 
 // the instantiation for this translation unit's activation; hid_ = the width decoded from `hidden`
 #define PROMP_DISPATCH_ACT(FN, DO, DA, HID, ...) return FN<DO, DA, HID, PROMP_POLICY_ACT>(__VA_ARGS__);
@@ -1283,41 +1326,27 @@ namespace PROMP_ACT_NS {
     const int hid_ = hidden & PROMP_HIDDEN_WIDTH_MASK;                          \
     if (padded) PROMP_DISPATCH_BUCKETS(FN, __VA_ARGS__)                          \
     PROMP_DISPATCH_DIMS(FN, __VA_ARGS__)
-int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_grad_any, A, ws, ws_bytes, s)
+int grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_grad_any, A, nh, ws, ws_bytes, s)
 }
-int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_hvp, A, ws, ws_bytes, s)
+int hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_hvp, A, nh, ws, ws_bytes, s)
 }
-int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns,
-                              int M) {
-    PROMP_DISPATCH(chain_ws_bytes, n_stages, kinds, Ns, M)
+int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds,
+                              const int* Ns, int M) {
+    PROMP_DISPATCH(chain_ws_bytes, n_stages, kinds, Ns, M, nh)
 }
-int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M) {
-    PROMP_DISPATCH(chain_num_launches, n_stages, kinds, Ns, M)
+int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, const int* Ns,
+                   int M) {
+    PROMP_DISPATCH(chain_num_launches, n_stages, kinds, Ns, M, nh)
 }
-int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A, const int* skip_flag,
-          const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_chain, n_stages, kinds, A, skip_flag, skip_theta, ws, ws_bytes, s)
+int chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,
+          const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s) {
+    PROMP_DISPATCH(launch_chain, n_stages, kinds, A, nh, skip_flag, skip_theta, ws, ws_bytes, s)
 }
-int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride, const float* obs,
-            float* mean, cudaStream_t s) {
-    PROMP_DISPATCH(launch_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, s)
-}
-// policies of depth 1 and 3 (policy_deep.cuh); nh = depth - 1
-int deep_grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_deep_grad, A, nh, ws, ws_bytes, s)
-}
-int deep_hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_deep_hvp, A, nh, ws, ws_bytes, s)
-}
-int deep_chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,
-               const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s) {
-    PROMP_DISPATCH(launch_deep_chain, n_stages, kinds, A, nh, skip_flag, skip_theta, ws, ws_bytes, s)
-}
-int deep_forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params, int64_t stride,
-                 const float* obs, float* mean, cudaStream_t s) {
-    PROMP_DISPATCH(launch_deep_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, nh, s)
+int forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params, int64_t stride,
+            const float* obs, float* mean, cudaStream_t s) {
+    PROMP_DISPATCH(launch_forward, M, N, params, stride, obs, mean, obs_dim, act_dim, nh, s)
 }
 }  // namespace PROMP_ACT_NS
 
@@ -1325,23 +1354,16 @@ int deep_forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int 
 // the dispatch of the other units: relu_tu (policy_relu.cu), otanh_tu (policy_otanh.cu), relu_otanh_tu (policy_relu_otanh.cu)
 #define PROMP_DECLARE_UNIT(NS)                                                                                                    \
     namespace NS {                                                                                                                \
-    int grad(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);       \
-    int hvp(bool padded, int obs_dim, int act_dim, int hidden, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);        \
-    int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds,              \
+    int grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s);\
+    int hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes, cudaStream_t s); \
+    int64_t chain_workspace_bytes(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds,      \
                                   const int* Ns, int M);                                                                          \
-    int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, const int* Ns, int M);  \
-    int chain(bool padded, int obs_dim, int act_dim, int hidden, int n_stages, const int* kinds, PolicyArgs* A,                   \
+    int chain_launches(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, const int* Ns,  \
+                       int M);                                                                                                    \
+    int chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,           \
               const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);                         \
-    int forward(bool padded, int obs_dim, int act_dim, int hidden, int M, int N, const float* params, int64_t stride,             \
+    int forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params, int64_t stride,     \
                 const float* obs, float* mean, cudaStream_t s);                                                                   \
-    int deep_grad(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes,           \
-                  cudaStream_t s);                                                                                                \
-    int deep_hvp(bool padded, int obs_dim, int act_dim, int hidden, int nh, PolicyArgs& A, void* ws, int64_t ws_bytes,            \
-                 cudaStream_t s);                                                                                                 \
-    int deep_chain(bool padded, int obs_dim, int act_dim, int hidden, int nh, int n_stages, const int* kinds, PolicyArgs* A,      \
-                   const int* skip_flag, const float* skip_theta, void* ws, int64_t ws_bytes, cudaStream_t s);                    \
-    int deep_forward(bool padded, int obs_dim, int act_dim, int hidden, int nh, int M, int N, const float* params,                \
-                     int64_t stride, const float* obs, float* mean, cudaStream_t s);                                              \
     }
 PROMP_DECLARE_UNIT(relu_tu)
 PROMP_DECLARE_UNIT(otanh_tu)
@@ -1363,17 +1385,7 @@ PROMP_DECLARE_UNIT(relu_otanh_tu)
 using namespace promp;
 
 extern "C" int64_t promp_policy_workspace_bytes(int M, int N, int obs_dim, int act_dim, int hidden) {
-    // upper bound over the occupancies the kernels can have (1..4 CTAs per SM on this device's SMs, or on 160)
-    const int P = promp_num_params(obs_dim, act_dim, hidden);
-    int64_t worst = 0;
-    for (int occ = 1; occ <= 4; ++occ)
-        for (int tb : {TB, TBT}) {            // CUDA-core kernels tile by 64 samples, the tensor-core kernels by 128
-            const TilePlan p = plan_tiles(M, N, 160 * occ, P, tb);
-            if (p.partial_floats > worst) worst = p.partial_floats;
-            const TilePlan p2 = plan_tiles(M, N, sm_count() * occ, P, tb);
-            if (p2.partial_floats > worst) worst = p2.partial_floats;
-        }
-    return counters_bytes(M) + worst * (int64_t)sizeof(float) + 16;
+    return policy_workspace_bytes(M, N, promp_num_params(obs_dim, act_dim, hidden));
 }
 
 extern "C" int promp_policy_layout(int obs_dim, int act_dim, int hidden, int32_t out[4]) {
@@ -1439,8 +1451,7 @@ static int policy_grad_impl(bool padded, int obs_dim, int act_dim, int hidden, i
     explore_args(A);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_grad")
-    if (depth_ != 2) return PROMP_UNIT(deep_grad)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
-    return PROMP_UNIT(grad)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
+    return PROMP_UNIT(grad)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_GRAD_EX_PARAMS                                                                                               \
@@ -1499,8 +1510,7 @@ static int policy_hvp_impl(bool padded, int obs_dim, int act_dim, int hidden, in
     A.obs_dim = obs_dim; A.act_dim = act_dim;
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_hvp")
-    if (depth_ != 2) return PROMP_UNIT(deep_hvp)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
-    return PROMP_UNIT(hvp)(padded, obs_dim, act_dim, hidden, A, workspace, workspace_bytes, s);
+    return PROMP_UNIT(hvp)(padded, obs_dim, act_dim, hidden, depth_ - 1, A, workspace, workspace_bytes, s);
 }
 
 #define PROMP_HVP_RAGGED_PARAMS                                                                                            \
@@ -1595,14 +1605,7 @@ static int64_t policy_chain_workspace_bytes_impl(bool padded, int obs_dim, int a
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_workspace_bytes")
-    if (depth_ != 2) {      // one launch per stage: the control words, then the workspace of the largest stand-alone launch
-        int nmax = 1;
-        for (int k = 0; k < n_stages; ++k) nmax = Ns[k] > nmax ? Ns[k] : nmax;
-        const int64_t single = padded ? promp_policy_workspace_bytes_padded(M, nmax, obs_dim, act_dim, hidden)
-                                      : promp_policy_workspace_bytes(M, nmax, obs_dim, act_dim, hidden);
-        return single < 0 ? -1 : chain_ctrl_bytes(M) + single;
-    }
-    return PROMP_UNIT(chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
+    return PROMP_UNIT(chain_workspace_bytes)(padded, obs_dim, act_dim, hidden, depth_ - 1, n_stages, kinds, Ns, M);
 }
 extern "C" int64_t promp_policy_chain_workspace_bytes(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                       const promp_policy_stage* stages) {
@@ -1619,8 +1622,7 @@ static int policy_chain_num_launches_impl(bool padded, int obs_dim, int act_dim,
     int kinds[CHAIN_MAX_STAGES], Ns[CHAIN_MAX_STAGES];
     for (int s = 0; s < n_stages; ++s) kinds[s] = stages[s].kind, Ns[s] = stages[s].N > 0 ? stages[s].N : 1;
     PROMP_DECODE_HIDDEN("promp_policy_chain_num_launches")
-    if (depth_ != 2) return n_stages;
-    return PROMP_UNIT(chain_launches)(padded, obs_dim, act_dim, hidden, n_stages, kinds, Ns, M);
+    return PROMP_UNIT(chain_launches)(padded, obs_dim, act_dim, hidden, depth_ - 1, n_stages, kinds, Ns, M);
 }
 extern "C" int promp_policy_chain_num_launches(int obs_dim, int act_dim, int hidden, int M, int n_stages,
                                                const promp_policy_stage* stages) {
@@ -1669,10 +1671,7 @@ static int policy_chain_impl(bool padded, int obs_dim, int act_dim, int hidden, 
     }
     const int rc_clear = chain_clear_on_new_m(workspace, M, s);
     if (rc_clear != PROMP_OK) return rc_clear;
-    if (depth_ != 2)
-        return PROMP_UNIT(deep_chain)(padded, obs_dim, act_dim, hidden, depth_ - 1, n_stages, kinds, A, skip_flag, skip_theta,
-                                      workspace, workspace_bytes, s);
-    return PROMP_UNIT(chain)(padded, obs_dim, act_dim, hidden, n_stages, kinds, A, skip_flag, skip_theta, workspace,
+    return PROMP_UNIT(chain)(padded, obs_dim, act_dim, hidden, depth_ - 1, n_stages, kinds, A, skip_flag, skip_theta, workspace,
                              workspace_bytes, s);
 }
 extern "C" int promp_policy_chain(int obs_dim, int act_dim, int hidden, int M, float min_log_std, int n_stages,
@@ -1722,8 +1721,7 @@ static int policy_forward_impl(bool padded, int obs_dim, int act_dim, int hidden
     PROMP_REQUIRE(M <= 65535, "promp_policy_forward: M=%d exceeds the grid.y limit", M);
     cudaStream_t s = (cudaStream_t)stream;
     PROMP_DECODE_HIDDEN("promp_policy_forward")
-    if (depth_ != 2) return PROMP_UNIT(deep_forward)(padded, obs_dim, act_dim, hidden, depth_ - 1, M, N, params, param_stride, obs, mean, s);
-    return PROMP_UNIT(forward)(padded, obs_dim, act_dim, hidden, M, N, params, param_stride, obs, mean, s);
+    return PROMP_UNIT(forward)(padded, obs_dim, act_dim, hidden, depth_ - 1, M, N, params, param_stride, obs, mean, s);
 }
 extern "C" int promp_policy_forward(int obs_dim, int act_dim, int hidden, int M, int N, const float* params,
                                     int64_t param_stride, const float* obs, float* mean, void* stream) {

@@ -1,7 +1,7 @@
 // CUDA-core kernels of the policies with one or three hidden layers (hidden_sizes of length 1 or 3, PROMP_HIDDEN_DEPTH):
 // gradient (with the E-MAML exploration variant), Hessian-vector product and forward.  Included by policy.cu after its
-// launch helpers, so that every activation unit (tanh_tu, relu_tu, otanh_tu, relu_otanh_tu) instantiates them for its own
-// activation; the two-layer kernels above are untouched.
+// two-layer kernels, so that every activation unit (tanh_tu, relu_tu, otanh_tu, relu_otanh_tu) instantiates them for its
+// own activation; policy.cu's launchers pick them for every depth but two.
 //
 // One instantiation per (obs, act, hidden width, activation) serves both depths: the number of hidden-to-hidden layers
 // nh = depth - 1 (0 or 2) is a kernel argument, the per-layer loops are unrolled to DEEP_NH and predicated on it.  The tile
@@ -873,85 +873,6 @@ __global__ void __launch_bounds__(128) policy_forward_deep_kernel(int M, int N, 
         }
         __syncwarp();
     }
-}
-
-// ------------------------------------------------------------------------------------------------------------ launches
-template <typename Kernel>
-static int launch_deep(Kernel kernel, int smem, int& occ_cache, PolicyArgs& A, int nh, int P, void* ws, int64_t ws_bytes,
-                       cudaStream_t st, const char* name) {
-    if (occ_cache == 0) {
-        PROMP_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        int occ = 0;
-        PROMP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, PT_THREADS, smem));
-        occ_cache = occ < 1 ? 1 : occ;
-    }
-    const TilePlan p = plan_tiles(A.M, A.N, sm_count() * occ_cache, P, TB);
-    const int64_t need = counters_bytes(A.M) + p.partial_floats * (int64_t)sizeof(float);
-    if (ws_bytes < need) {
-        set_error("policy workspace too small (%lld < %lld bytes)", (long long)ws_bytes, (long long)need);
-        return PROMP_ERR_WORKSPACE;
-    }
-    A.counters = (int*)ws;
-    A.partial = (float*)((char*)ws + counters_bytes(A.M));
-    A.q = p.q;
-    A.kmax = p.kmax;
-    kernel<<<p.grid, PT_THREADS, smem, st>>>(A, nh);
-    PROMP_LAUNCH_CHECK(name);
-    return PROMP_OK;
-}
-
-template <int DO, int DA, int HID, class Act>
-static int launch_deep_grad(PolicyArgs& A, int nh, void* ws, int64_t ws_bytes, cudaStream_t st) {
-    const int P = DeepLayout<DO, DA, HID>{nh}.P();
-    constexpr int smem = (int)sizeof(DeepGradSmem<DO, DA, HID>);
-    if (A.adv_per_task) {
-        static int occ_x = 0;
-        return launch_deep(policy_grad_deep_kernel<DO, DA, HID, Act, ADV_TASK>, smem, occ_x, A, nh, P, ws, ws_bytes, st,
-                           "policy_grad_deep_kernel");
-    }
-    static int occ = 0;
-    return launch_deep(policy_grad_deep_kernel<DO, DA, HID, Act, ADV_SAMPLE>, smem, occ, A, nh, P, ws, ws_bytes, st,
-                       "policy_grad_deep_kernel");
-}
-
-template <int DO, int DA, int HID, class Act>
-static int launch_deep_hvp(PolicyArgs& A, int nh, void* ws, int64_t ws_bytes, cudaStream_t st) {
-    static_assert(sizeof(DeepHvpSmem<DO, DA, HID>) <= 227 * 1024, "deep HVP tile exceeds the shared memory of one SM");
-    static int occ = 0;
-    return launch_deep(policy_hvp_deep_kernel<DO, DA, HID, Act>, (int)sizeof(DeepHvpSmem<DO, DA, HID>), occ, A, nh,
-                       DeepLayout<DO, DA, HID>{nh}.P(), ws, ws_bytes, st, "policy_hvp_deep_kernel");
-}
-
-// The chain's stages as one launch each (the dataflow kernel is built for two hidden layers); workspace as launch_chain's
-// one-launch-per-stage path
-template <int DO, int DA, int HID, class Act>
-static int launch_deep_chain(int n_stages, const int* kinds, PolicyArgs* A, int nh, const int* skip_flag, const float* skip_theta,
-                             void* ws, int64_t ws_bytes, cudaStream_t st) {
-    const int M = A[0].M;
-    const int64_t off1 = chain_ctrl_bytes(M) - counters_bytes(M);
-    void* ws1 = (char*)ws + off1;
-    const int64_t ws1_bytes = ws_bytes - off1;
-    for (int s = 0; s < n_stages; ++s) {
-        PolicyArgs a = A[s];
-        if (s == 0) a.skip_flag = skip_flag, a.skip_theta = skip_theta;
-        const int rc = kinds[s] == 0 ? launch_deep_grad<DO, DA, HID, Act>(a, nh, ws1, ws1_bytes, st)
-                                     : launch_deep_hvp<DO, DA, HID, Act>(a, nh, ws1, ws1_bytes, st);
-        if (rc != PROMP_OK) return rc;
-    }
-    return PROMP_OK;
-}
-
-template <int DO, int DA, int HID, class Act>
-static int launch_deep_forward(int M, int N, const float* params, int64_t stride, const float* obs, float* mean, int obs_dim,
-                               int act_dim, int nh, cudaStream_t st) {
-    int gx = (N + 3) / 4;
-    const int cap = (4 * sm_count() + M - 1) / M;
-    if (gx > cap) gx = cap;
-    if (gx < 1) gx = 1;
-    policy_forward_deep_kernel<DO, DA, HID, Act><<<dim3(gx, M), 128, 0, st>>>(M, N, params, stride, obs, mean, obs_dim, act_dim,
-                                                                               nh);
-    PROMP_LAUNCH_CHECK("policy_forward_deep_kernel");
-    return PROMP_OK;
 }
 
 }  // namespace promp
