@@ -163,6 +163,14 @@ int promp_rollout_ex(int env_kind, int reward_type, float sparse_radius, int nor
 int promp_counter_add(uint64_t* counter, uint64_t inc, void* stream);
 
 /*
+ * Set the tasks of a sampling phase: per_task [M, task_dim] = host_vec (host memory, read during the call) and, when
+ * per_env is not NULL, per_env [M * E, task_dim] = each task's row repeated for its E envs.  The values travel in the
+ * kernel arguments (960 per launch), so the call never waits for work already queued on the stream and host_vec may be
+ * reused as soon as it returns.
+ */
+int promp_set_tasks(int M, int task_dim, int E, const float* host_vec, float* per_task, float* per_env, void* stream);
+
+/*
  * One vectorised env step (MetaIterativeEnvExecutor.step, samplers/vectorized_env_executor.py:25-52)
  * for policies that are not device-resident: state [n_env, state_dim] is updated in place.
  *   actions [n_env, Da] policy-space actions (NormalizedEnv rescale+clip applied inside when normalize_actions = 1)

@@ -66,6 +66,7 @@ _SIGNATURES = {
     'promp_paths_finalize_ex': (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int64, _P, _P, _P, _P, _P, _P, _P, _P,
                                         _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P]),
     'promp_counter_add': (c_int, [_P, c_uint64, _P]),
+    'promp_set_tasks': (c_int, [c_int, c_int, c_int, _P, _P, _P, _P]),
     'promp_env_step': (c_int, [c_int, c_int, c_float, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     'promp_env_observe': (c_int, [c_int, c_int, _P, _P, _P]),
     'promp_process_workspace_bytes': (c_int64, [c_int, c_int, c_int, c_int]),

@@ -1,5 +1,6 @@
 // Launch dispatch and C entry points of the fused rollout kernel and the single-step vec-env kernels (rollout_kernel.cuh).
 // See include/promp_b200.h for the interface and the reference functions each entry point replaces.
+#include <cstring>
 #include <type_traits>
 
 #include "rollout_kernel.cuh"
@@ -213,6 +214,43 @@ extern "C" int promp_counter_add(uint64_t* counter, uint64_t inc, void* stream) 
     PROMP_REQUIRE(counter != nullptr, "promp_counter_add: null counter");
     counter_add_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(counter, inc);
     PROMP_LAUNCH_CHECK("counter_add_kernel");
+    return PROMP_OK;
+}
+
+// The task vectors travel inside the kernel's argument block, which the launch copies when it is enqueued: no host memory
+// has to outlive the call and nothing waits for the stream.  A copy from pageable memory would wait for all work queued
+// before it, and the device would then idle while the host enqueues what follows.  SET_TASKS_CHUNK floats per launch keep
+// the block under the 4 KB kernel parameter limit.
+constexpr int SET_TASKS_CHUNK = 960;
+struct SetTasksArgs {
+    float v[SET_TASKS_CHUNK];      // per-task values [c0, c0 + n) of the flat [M, task_dim] array
+    int c0, n, task_dim, E;
+    float* per_task;               // [M, task_dim]
+    float* per_env;                // [M * E, task_dim] or NULL
+};
+__global__ void set_tasks_kernel(const __grid_constant__ SetTasksArgs A) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;        // (value, env of its task) pairs, value-major
+    const int E = A.per_env ? A.E : 1;
+    if (i >= A.n * E) return;
+    const int j = i / E, k = i - j * E;
+    const int f = A.c0 + j, m = f / A.task_dim, d = f - m * A.task_dim;
+    if (k == 0) A.per_task[f] = A.v[j];
+    if (A.per_env) A.per_env[((int64_t)m * A.E + k) * A.task_dim + d] = A.v[j];
+}
+extern "C" int promp_set_tasks(int M, int task_dim, int E, const float* host_vec, float* per_task, float* per_env,
+                               void* stream) {
+    PROMP_REQUIRE(M >= 0 && task_dim > 0 && E > 0, "promp_set_tasks: M >= 0, task_dim > 0 and E > 0 required");
+    PROMP_REQUIRE(M == 0 || (host_vec && per_task), "promp_set_tasks: null host_vec or per_task");
+    const int64_t total = (int64_t)M * task_dim;
+    for (int64_t c0 = 0; c0 < total; c0 += SET_TASKS_CHUNK) {
+        SetTasksArgs A;
+        A.n = (int)(total - c0 < SET_TASKS_CHUNK ? total - c0 : SET_TASKS_CHUNK);
+        A.c0 = (int)c0, A.task_dim = task_dim, A.E = E, A.per_task = per_task, A.per_env = per_env;
+        memcpy(A.v, host_vec + c0, sizeof(float) * A.n);
+        const int64_t threads = (int64_t)A.n * (per_env ? E : 1);
+        set_tasks_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(A);
+        PROMP_LAUNCH_CHECK("set_tasks_kernel");
+    }
     return PROMP_OK;
 }
 

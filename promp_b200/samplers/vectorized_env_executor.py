@@ -44,14 +44,16 @@ class MetaDeviceEnvExecutor(object):
         return self.n_envs
 
     def set_tasks(self, tasks):
-        """vectorized_env_executor.py:54-64."""
-        import torch
+        """vectorized_env_executor.py:54-64.  One launch carries the task vectors (promp_set_tasks): the host does not wait for
+        the work already queued, such as the previous iteration's graph replay."""
         assert len(tasks) == self.meta_batch_size
         self.tasks = list(tasks)
         inner = getattr(self.env, '_wrapped_env', self.env)
-        vec = np.stack([inner.task_vector(t) for t in tasks]).astype(np.float32)
-        self.task_params_per_task.copy_(torch.from_numpy(vec))
-        self.task_params.copy_(self.task_params_per_task.repeat_interleave(self.envs_per_task, dim=0))
+        vec = np.ascontiguousarray(np.stack([inner.task_vector(t) for t in tasks]), dtype=np.float32)
+        assert vec.size == self.task_params_per_task.numel(), "task vectors of %d values, expected %d" % (
+            vec.size, self.task_params_per_task.numel())
+        _lib.call('promp_set_tasks', self.meta_batch_size, self.spec['task_dim'], self.envs_per_task, vec.ctypes.data,
+                  _lib.ptr(self.task_params_per_task), _lib.ptr(self.task_params), _lib.stream())
         if len(tasks):
             self.env.set_task(tasks[-1])
 
